@@ -16,14 +16,18 @@ model API, wrapper tiling/chunking on.  Configs (BASELINE.json `configs[1..4]`):
 Keys:
   value      frames/s, inputs resident in HBM when the timed region starts
   e2e        same through host buffers: pinned host clip -> H2D -> encode/decode -> D2H of the reconstruction, per step
-  roofline   tensor bound of the dominant kernels (tcgen05 implicit-GEMM conv): algorithmic FLOPs of their launches /
-             their CUDA-event time in the timed region, against MEASURED_PEAKS.json (sustained bf16 cuBLAS TF/s)
+  roofline   tensor bound of the dominant kernels (wgmma implicit-GEMM conv): algorithmic FLOPs of their launches /
+             their CUDA-event time in the timed region, against MEASURED_PEAKS.json (sustained bf16 TF/s) when present,
+             else the H100 SXM data-sheet dense fp16/bf16 rate (989 TF/s at 700 W)
   cpu_baseline        the oracle (CPU restatement of the reference algorithm, fp32) on the host cores, on a bounded
              sample, scaled to the workload by network-input pixel count            (N = 1, rank 0)
   torch_cuda_baseline the reference ALGORITHM in the bench dtype on torch-CUDA library kernels (cuDNN / SDPA), eager,
              wrapper tiling on, cudnn.benchmark False and True - the north_star's ">= 4x" denominator (N = 1, c2/c3)
   parity_sharded      N > 1: rank 0 also runs the un-sharded clip and the gathered sharded result must be
              bit-identical (moments and reconstruction); the line carries the verdict
+--dump-outputs DIR writes what the last timed step computed (rank 0): latent.npy (the latents fed to the decoder) and
+reconstruction.npy, float32; an output larger than 7.5 M values is replaced by a fixed seeded sample of 7.5 M of its
+values (flattened order), so two builds run with the same arguments can be compared value for value.
 """
 from __future__ import annotations
 
@@ -59,7 +63,7 @@ CONFIGS = {
 def parse():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--steps", type=int, default=5, help="timed steps (>= 1)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference", "torch-cuda"])
     ap.add_argument("--config", default="c2", choices=sorted(CONFIGS))
@@ -74,7 +78,11 @@ def parse():
                     help="N > 1, batch-1 configs: 'frame' = clip sharded on the frame axis + halo exchange (default; c2/c3 grow the "
                          "clip with N), 'unit' = the FIXED clip resident on every rank, its (chunk x tile) work units dealt over "
                          "the ranks (strong scaling of a clip with fewer chunks than GPUs)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's latents and reconstruction to DIR/<name>.npy (float32, <= 64 MB in all)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     cfg = dict(CONFIGS[args.config])
     for k in ("frames", "height", "width", "dtype"):
         if getattr(args, k) is not None:
@@ -89,8 +97,8 @@ def peaks():
     if os.path.exists(p):
         with open(p) as f:
             d = json.load(f)
-        return float(d.get("bf16_tflops_sustained", 1400.0)), "MEASURED_PEAKS.json bf16_tflops_sustained (of measured)"
-    return 1400.0, "fallback 1.4 PFLOP/s sustained (of fallback)"
+        return float(d.get("bf16_tflops_sustained", 989.0)), "MEASURED_PEAKS.json bf16_tflops_sustained (of measured)"
+    return 989.0, "H100 SXM data sheet, dense fp16/bf16 at 700 W (not a measured peak)"
 
 
 def source_hash(root=None):
@@ -273,7 +281,7 @@ def build_model(cfg, dtype):
 
 class TorchCudaReference:
     """The reference algorithm on torch-CUDA library kernels (cuDNN etc.): the north_star's '>= 4x the reference's own
-    torch-cuda' denominator.  The reference is Python and /root/reference does not exist on the GPU box, so this runs its
+    torch-cuda' denominator.  The reference's own Python modules are not part of this repository, so this runs its
     pinned restatement (oracle/, checked against the reference's own outputs in tests/test_oracle_golden.py) with the
     same state dict as the engine; kind = "port"."""
 
@@ -318,6 +326,22 @@ def time_torch_cuda(ref, x, zc, warmup=3, reps=10):
     torch.backends.cudnn.benchmark = False
     torch.cuda.empty_cache()
     return out
+
+
+DUMP_MAX_VALUES = 7_500_000   # per output: 2 x 30 MB of float32 at most
+
+
+def dump_outputs(arrays, out_dir):
+    """arrays -> out_dir/<name>.npy as float32; larger outputs as a sample at fixed seeded positions (flattened order)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        flat = t.detach().reshape(-1)
+        if flat.numel() > DUMP_MAX_VALUES:
+            g = torch.Generator().manual_seed(0)
+            idx = torch.randint(0, flat.numel(), (DUMP_MAX_VALUES,), generator=g).sort().values
+            flat = flat[idx.to(flat.device)]
+        np.save(os.path.join(out_dir, name + ".npy"), flat.float().cpu().numpy())
 
 
 def main():
@@ -403,15 +427,21 @@ def main():
     x_host = gen_chunk_frames(f0, f1, seed_base=(rank * 100 if (sharded is None and unit is None and world > 1) else 0)).pin_memory()
     x_dev = x_host.cuda()
 
+    last = {}   # what the latest step computed, for --dump-outputs
+
     def step(x):
         with torch.no_grad():
             if sharded is not None:
                 z = sharded.encode_local(x, total_chunks)[:, :zc].contiguous()
-                return sharded.decode_local(z, total_chunks)
-            if unit is not None:
-                return unit.decode(unit.encode(x)[:, :zc].contiguous())
-            z = net.tiled_encode(x)[:, :zc]
-            return net.tiled_decode(z)
+                rec = sharded.decode_local(z, total_chunks)
+            elif unit is not None:
+                z = unit.encode(x)[:, :zc].contiguous()
+                rec = unit.decode(z)
+            else:
+                z = net.tiled_encode(x)[:, :zc]
+                rec = net.tiled_decode(z)
+        last["latent"], last["reconstruction"] = z, rec
+        return rec
 
     def sync():
         torch.cuda.synchronize()
@@ -493,6 +523,8 @@ def main():
     ms_per_rank = getattr(timed, "per_rank", None)
     prof = ops.stop_profile() if ops else None
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(last, args.dump_outputs)
     launches = (ops.launch_count() - launches0) if ops else 0
     ms_step = ms_total / args.steps
     job_frames = B * total_frames
@@ -528,19 +560,9 @@ def main():
     if prof and prof["conv_tc"]["ms"] > 0:
         tc = prof["conv_tc"]
         achieved = tc["flops"] / (tc["ms"] * 1e-3) / 1e12
-        traffic, traffic_src, traffic_stale = None, None, None
-        tp = os.path.join(ROOT, "profiles", "r02_traffic.json")
-        if os.path.exists(tp) and args.config == "c2":
-            # ncu dram bytes (read + write) per conv launch of this command, from the committed capture; stamped with the
-            # hash of the CUDA sources it was captured from - a mismatch means the kernels changed since (stale)
-            with open(tp) as f:
-                tj = json.load(f)
-            traffic, traffic_src = tj["dram_bytes_per_launch"], tj["source"]
-            traffic_stale = tj.get("source_hash") != source_hash()
-        roof = {"bound": "tensor", "kernel": "conv_tc_kernel / conv_tc_psw_kernel / conv_stk_kernel (tcgen05 implicit-GEMM conv, all "
-                                             "launches of the timed region)",
-                "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak, "traffic": traffic,
-                "traffic_source": traffic_src, "traffic_stale": traffic_stale,
+        roof = {"bound": "tensor", "kernel": "conv_tc_kernel / conv_stk_kernel (wgmma implicit-GEMM conv, all launches of the "
+                                             "timed region)",
+                "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
                 "algorithmic_bytes_per_launch": tc["bytes"] / max(tc["launches"], 1),
                 "peak_source": peak_src, "algorithmic_tflop_per_step": tc["flops"] / args.steps / 1e12,
                 "kernel_ms_per_step": tc["ms"] / args.steps, "launches_per_step": tc["launches"] / args.steps,
@@ -562,13 +584,13 @@ def main():
                                    f"seeded random weights",
                        "per_gpu": f"{b_local} x {c1 - c0} chunk(s) of <= 17 frames x {n_tiles} spatial tile(s) (<= 576x576, stride 448)",
                        "parallelism": par,
-                       "l2": "no explicit flush: every step streams far more than the 126 MB L2 (activations up to 1.4 GB each)"},
+                       "l2": "no explicit flush: every step streams far more than the 50 MB L2 (activations up to 1.4 GB each)"},
             "impl": args.impl, "gpu_launches": launches // args.steps if launches else 0, "clocks": clocks, "e2e": e2e,
             "peak_hbm_gb": peak_hbm, "source_hash": source_hash()}
     if parity is not None:
         line["parity_sharded"] = parity
     if ms_per_rank is not None:
-        # `ms_per_step` is the MAX of these (the slowest GPU sets the pace of a weak-scaled job; power-capped B200s of one box
+        # `ms_per_step` is the MAX of these (the slowest GPU sets the pace of a weak-scaled job; power-capped GPUs of one box
         # differ by a few per cent)
         line["ms_per_step_per_rank"] = ms_per_rank
     if roof:
@@ -580,7 +602,7 @@ def main():
             tcb.update({"kind": "port", "unit": UNIT, "dtype": args.dtype,
                         "what": "reference algorithm (oracle restatement pinned to the reference's outputs) on torch-CUDA library "
                                 "kernels, eager, wrapper tiling/chunking on, same state dict and input; CUDA events, 3 warm-ups, "
-                                "median of 10; the reference's own modules cannot travel to the GPU box (/root/reference absent)"})
+                                "median of 10; the reference's own modules are not part of this repository"})
             tcb["speedup_value_vs_cudnn_benchmark_false"] = value / tcb["cudnn_benchmark_false"]["frames_per_s"]
             tcb["speedup_value_vs_cudnn_benchmark_true"] = value / tcb["cudnn_benchmark_true"]["frames_per_s"]
             line["torch_cuda_baseline"] = tcb

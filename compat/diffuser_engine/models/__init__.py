@@ -1,1 +1,1 @@
-"""`models` package name of the reference checkout, resolved to the B200 engine (see compat/README.md)."""
+"""`models` package name of the reference checkout, resolved to the H100 engine (see compat/README.md)."""

@@ -1,4 +1,4 @@
-"""cvvae_b200 - B200-native (sm_100a) implementation of the CV-VAE encode()/decode() hot path.
+"""cvvae_b200 - H100-native (sm_90a) implementation of the CV-VAE encode()/decode() hot path.
 
 Public surface (mirrors the reference's models/modeling_vae.py):
     CVVAEModel, CVVAESD3Model

@@ -1,7 +1,7 @@
-"""In-tree build of libcvvae_b200.so (nvcc, sm_100a only).
+"""In-tree build of libcvvae_b200.so (nvcc, sm_90a only).
 
-The shared object lands in ``cvvae_b200/lib/`` so that it travels with a repository snapshot to the
-GPU box; nothing is installed into site-packages and no JIT cache is used.
+The shared object lands in ``cvvae_b200/lib/`` inside the tree, so the package imports from the repository;
+nothing is installed into site-packages and no JIT cache is used.
 """
 from __future__ import annotations
 
@@ -16,7 +16,7 @@ LIBDIR = os.path.join(HERE, "lib")
 LIBPATH = os.path.join(LIBDIR, "libcvvae_b200.so")
 SOURCES = ["api.cu", "conv_tc.cu", "conv_stk.cu", "conv_direct.cu", "groupnorm.cu", "attention.cu", "misc.cu", "video_io.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC",
 ]
 
@@ -37,7 +37,7 @@ def _stale() -> bool:
 
 
 def build_library(force: bool = False, verbose: bool = False) -> str:
-    """Compile every CUDA source for sm_100a and link the C-ABI shared library. Returns its path."""
+    """Compile every CUDA source for sm_90a and link the C-ABI shared library. Returns its path."""
     if not force and not _stale():
         return LIBPATH
     nvcc = _nvcc()

@@ -1,5 +1,5 @@
 // Library-wide state of libcvvae_b200 (error string, launch counter, driver entry point) and the
-// UMMA descriptor probe used by the GPU test-suite.
+// shared-memory matrix descriptor probe used by the GPU test-suite.
 #include <stdarg.h>
 #include <string.h>
 
@@ -32,66 +32,58 @@ PFN_encodeTiled get_encode_tiled() {
   return fn;
 }
 
-// One CTA: TMA a [rows_total][64] 16-bit matrix and a [n][64] matrix into SWIZZLE_128B shared memory, run a
-// single 128 x n x 64 UMMA whose A descriptor starts `row_shift` rows (128 B each) into the slab and whose 8-row
-// groups are `sbo_rows` rows apart (8 = dense; 16 = every other group, i.e. a tile of 8-position image rows cut out
-// of a wider slab).
+// One warpgroup: TMA a [rows_total][64] 16-bit matrix and a [N][64] matrix into SWIZZLE_128B shared memory, run a
+// 128 x N x 64 product as two 64-row wgmma chains whose A descriptor starts `row_shift` rows (128 B each) into the slab
+// and whose 8-row groups are `sbo_rows` rows apart (8 = dense; 16 = every other group, i.e. a tile of 8-position image
+// rows cut out of a wider slab).
+template <int N>
 __global__ void __launch_bounds__(128) probe_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                    const __grid_constant__ CUtensorMap tmB, float* out, int n,
-                                                    int rows_total, int row_shift, int base_offset_mode, int sbo_rows) {
+                                                    const __grid_constant__ CUtensorMap tmB, float* out, int rows_total,
+                                                    int row_shift, int base_offset_mode, int sbo_rows) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;                  // rows_total * 128 B (<= 48 KB)
-  uint8_t* sB = smem + 49152;          // n * 128 B
+  uint8_t* sB = smem + 49152;          // N * 128 B
   uint64_t* bar = reinterpret_cast<uint64_t*>(smem + 49152 + 32768);
-  uint64_t* done = bar + 1;
-  uint32_t* slot = reinterpret_cast<uint32_t*>(bar + 2);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     ptx::mbar_init(bar, 1);
-    ptx::mbar_init(done, 1);
     ptx::fence_mbar_init();
   }
-  if (warp == 1) {
-    ptx::tmem_alloc(slot, 256);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem = *slot;
   if (threadIdx.x == 0) {
-    ptx::mbar_expect_tx(bar, static_cast<uint32_t>(rows_total + n) * 128u);
+    ptx::mbar_expect_tx(bar, static_cast<uint32_t>(rows_total + N) * 128u);
     ptx::tma_load_3d(sA, &tmA, bar, 0, 0, 0);                                   // two boxes of rows_total / 2 rows
     ptx::tma_load_3d(sA + (rows_total / 2) * 128, &tmA, bar, 0, rows_total / 2, 0);
     ptx::tma_load_3d(sB, &tmB, bar, 0, 0, 0);
-    ptx::mbar_wait(bar, 0);
-    ptx::tc_fence_after();
-    const uint32_t a0 = ptx::smem_u32(sA) + static_cast<uint32_t>(row_shift) * 128u;
-    const uint32_t b0 = ptx::smem_u32(sB);
-    const uint32_t bo = base_offset_mode ? ((a0 >> 7) & 7u) : 0u;
-    const uint32_t idesc = ptx::umma_idesc_f16(0, 128, n);
+  }
+  ptx::mbar_wait(bar, 0);
+  float acc[2][N / 2];
+  const uint32_t b0 = ptx::smem_u32(sB);
+  ptx::wgmma_fence();
+#pragma unroll
+  for (int c = 0; c < 2; ++c) {
+    const uint32_t a0 = ptx::smem_u32(sA) + static_cast<uint32_t>(row_shift + c * 8 * sbo_rows) * 128u;
+    const uint64_t bo = base_offset_mode ? static_cast<uint64_t>((a0 >> 7) & 7u) << 49 : 0ull;
+#pragma unroll
     for (int k = 0; k < 4; ++k)
-      ptx::umma_f16(tmem, ptx::umma_desc_k_sw128(a0 + k * 32, static_cast<uint32_t>(sbo_rows) * 128u, bo),
-                    ptx::umma_desc_k_sw128(b0 + k * 32, 1024), idesc, k > 0);
-    ptx::umma_commit(done);
+      ptx::Wgmma<CVVAE_F16, N>::run(acc[c], ptx::wgmma_desc_sw128(a0 + k * 32, static_cast<uint32_t>(sbo_rows) * 128u) | bo,
+                                    ptx::wgmma_desc_sw128(b0 + k * 32), k > 0);
   }
-  __syncwarp();
-  ptx::mbar_wait(done, 0);
-  ptx::tc_fence_after();
-  const int r = warp * 32 + lane;
-  for (int c0 = 0; c0 < n; c0 += 32) {
-    uint32_t v[32];
-    ptx::tmem_ld_32x32(tmem + (static_cast<uint32_t>(warp * 32) << 16) + c0, v);
-    ptx::tmem_ld_wait();
-    for (int j = 0; j < 32 && c0 + j < n; ++j) out[r * n + c0 + j] = __uint_as_float(v[j]);
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem, 256);
-  }
+  ptx::wgmma_commit();
+  ptx::wgmma_wait<0>();
+#pragma unroll
+  for (int c = 0; c < 2; ++c) ptx::fence_regs(acc[c]);
+#pragma unroll
+  for (int c = 0; c < 2; ++c)
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int r = c * 64 + warp * 16 + (lane >> 2) + (i >> 1) * 8;
+        const int col = 8 * j + 2 * (lane & 3) + (i & 1);
+        out[r * N + col] = acc[c][4 * j + i];
+      }
 }
 
 }  // namespace cvvae
@@ -104,7 +96,7 @@ extern "C" int64_t cvvae_launch_count(void) { return g_launches.load(); }
 
 extern "C" int cvvae_probe_umma_shift(const void* a_rows, const void* b_rows, float* out, int32_t n, int32_t row_shift,
                                       int32_t base_offset_mode, int32_t sbo_rows, void* stream_) {
-  CVVAE_CHECK_ARG(a_rows && b_rows && out && n >= 16 && n <= 256 && n % 16 == 0 && row_shift >= 0 && row_shift <= 64 &&
+  CVVAE_CHECK_ARG(a_rows && b_rows && out && (n == 64 || n == 128 || n == 256) && row_shift >= 0 && row_shift <= 64 &&
                       sbo_rows >= 8 && sbo_rows <= 16,
                   "cvvae_probe_umma_shift: bad argument");
   PFN_encodeTiled enc = get_encode_tiled();
@@ -131,9 +123,17 @@ extern "C" int cvvae_probe_umma_shift(const void* a_rows, const void* b_rows, fl
     CVVAE_CHECK_ARG(r == CUDA_SUCCESS, "probe: tensor map B failed (%d)", (int)r);
   }
   const size_t smem = 1024 + 49152 + 32768 + 64;
-  CVVAE_CUDA(cudaFuncSetAttribute(probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  probe_kernel<<<1, 128, smem, static_cast<cudaStream_t>(stream_)>>>(tmA, tmB, out, n, rows_total, row_shift, base_offset_mode,
-                                                                      sbo_rows);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (n == 64) {
+    CVVAE_CUDA(cudaFuncSetAttribute(probe_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    probe_kernel<64><<<1, 128, smem, stream>>>(tmA, tmB, out, rows_total, row_shift, base_offset_mode, sbo_rows);
+  } else if (n == 128) {
+    CVVAE_CUDA(cudaFuncSetAttribute(probe_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    probe_kernel<128><<<1, 128, smem, stream>>>(tmA, tmB, out, rows_total, row_shift, base_offset_mode, sbo_rows);
+  } else {
+    CVVAE_CUDA(cudaFuncSetAttribute(probe_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    probe_kernel<256><<<1, 128, smem, stream>>>(tmA, tmB, out, rows_total, row_shift, base_offset_mode, sbo_rows);
+  }
   CVVAE_LAUNCH_CHECK();
   return CVVAE_OK;
 }

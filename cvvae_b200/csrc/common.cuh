@@ -125,7 +125,7 @@ inline int num_sms() {
   int v = n[dev].load(std::memory_order_relaxed);
   if (v == 0) {
     cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    if (v <= 0) v = 148;
+    if (v <= 0) v = 132;
     n[dev].store(v, std::memory_order_relaxed);
   }
   return v;

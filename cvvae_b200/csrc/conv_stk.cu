@@ -1,13 +1,13 @@
 // Tap-stacked 3x3(x3) convolution for tiny Cout (the decoder's conv_out, 128 -> 3 at full resolution).
 //
-// With N = Cout padded to 16 the tensor core is idle: every 128x16x16 MMA still has to read its 4 KB A tile from shared
-// memory (64 cycles) for 8 cycles of math, and the ordinary kernel issues one such MMA per tap (3.3 ms per 17x576x576 tile).
+// With N = Cout padded to a minimal tile the tensor core is idle: every MMA still has to read its A tile from shared memory
+// for a few cycles of math, and the ordinary kernel issues one such MMA per tap.
 // Here the nine (kh,kw) taps are stacked along N instead: B = [9 taps x 8 channel slots (+8 pad) = 80 rows][64 K], and ONE
 // MMA on the UNSHIFTED slab tile produces, for every slab position, the partial sums of all nine taps; only the time
 // taps and the channel blocks remain in the K loop (KT x Cin/64 x 4 MMAs per sub-tile instead of 27 x ...).  The spatial
 // shifts are applied afterwards, on the tiny per-position partials, through a shared-memory exchange:
 //     y[h][w][c] = sum_{kh,kw} P[(kh,kw)][h+kh-1][w+kw-1][c].
-// Tile: a 16 x 32 slab of input positions (512 MMA rows, 4 sub-tiles) -> 14 x 30 outputs.
+// Tile: a 12 x 32 slab of input positions (384 MMA rows: 3 x 64 per MMA warpgroup) -> 10 x 30 outputs.
 //
 // Replaces cuDNN behind Decoder.conv_out (reference models/vae_models.py:942-944,999; vae_models3d_sd3.py:319,385).
 #include "common.cuh"
@@ -23,18 +23,19 @@ struct ConvStkParams {
   const float* bias;
   void* y;
   long long ys_b, ys_t, ys_h, ys_w, ys_c;
-  uint32_t idesc;
   int xstride;  // floats per slab position in the exchange buffer
 };
 
-static constexpr int kSlabW = 32, kSlabH = 16, kOutW = 30, kOutH = 14;
-static constexpr int kNstk = 80;                      // 9 taps x 8 channel slots + 8 rows of padding (UMMA N % 16 == 0)
-static constexpr uint32_t kSlabBytes = kSlabW * kSlabH * 128;  // 64 KB per 64-channel block
+static constexpr int kSlabW = 32, kSlabH = 12, kOutW = 30, kOutH = 10;
+static constexpr int kChunks = kSlabW * kSlabH / 128;   // 64-row MMA chunks per warpgroup (3 x 40 accumulator registers)
+static constexpr int kNstk = 80;                      // 9 taps x 8 channel slots + 8 rows of padding
+static constexpr uint32_t kSlabBytes = kSlabW * kSlabH * 128;  // 48 KB per 64-channel block
 static constexpr uint32_t kBBytes = kNstk * 128;      // 10 KB
 static constexpr int kNA = 2, kNB = 4;
+static constexpr int kStkThreads = 384;               // warpgroup 0: TMA producers; 1, 2: MMA + epilogue
 
 template <int DT>
-__global__ void __launch_bounds__(256, 1)
+__global__ void __launch_bounds__(kStkThreads, 1)
     conv_stk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const ConvStkParams p) {
   using E = Elem<DT>;
   extern __shared__ uint8_t smem_raw[];
@@ -46,8 +47,6 @@ __global__ void __launch_bounds__(256, 1)
   uint64_t* emptyA = bars + 4;
   uint64_t* fullB = bars + 8;
   uint64_t* emptyB = bars + 12;
-  uint64_t* accFull = bars + 16;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 17);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   int id = blockIdx.x;
@@ -57,21 +56,13 @@ __global__ void __launch_bounds__(256, 1)
   const int b = id / p.tiles_h;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < kNA; ++i) { ptx::mbar_init(&fullA[i], 1); ptx::mbar_init(&emptyA[i], 1); }
-    for (int i = 0; i < kNB; ++i) { ptx::mbar_init(&fullB[i], 1); ptx::mbar_init(&emptyB[i], 1); }
-    ptx::mbar_init(accFull, 1);
+    for (int i = 0; i < kNA; ++i) { ptx::mbar_init(&fullA[i], 1); ptx::mbar_init(&emptyA[i], 2); }
+    for (int i = 0; i < kNB; ++i) { ptx::mbar_init(&fullB[i], 1); ptx::mbar_init(&emptyB[i], 2); }
     ptx::fence_mbar_init();
     ptx::prefetch_tmap(&tmA);
     ptx::prefetch_tmap(&tmB);
   }
-  if (warp == 3) {
-    ptx::tmem_alloc(tmem_slot, 512);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   // the K loop: time taps (clamped or skipped at the clip ends) x 64-channel blocks
   auto for_each_step = [&](auto&& f) {
@@ -85,116 +76,120 @@ __global__ void __launch_bounds__(256, 1)
     }
   };
 
-  if (warp == 0) {
+  if (threadIdx.x < 128) {
+    ptx::setmaxnreg_dec<40>();
     int slot = 0;
     uint32_t phase = 0;
-    for_each_step([&](int kt, int ti, int cb) {
-      ptx::mbar_wait(&emptyA[slot], phase ^ 1);
-      if (ptx::elect_one()) {
-        ptx::mbar_expect_tx(&fullA[slot], kSlabBytes);
-        // slab position (0,0) is the input position of output (h0,w0) at tap (0,0)
-        ptx::tma_load_5d(sA + slot * kSlabBytes, &tmA, &fullA[slot], cb * 64, w0 + p.off_w, h0 + p.off_h, ti, b);
-      }
-      __syncwarp();
-      if (++slot == kNA) { slot = 0; phase ^= 1; }
-    });
-  } else if (warp == 1) {
-    int slot = 0;
-    uint32_t phase = 0;
-    for_each_step([&](int kt, int ti, int cb) {
-      ptx::mbar_wait(&emptyB[slot], phase ^ 1);
-      if (ptx::elect_one()) {
-        ptx::mbar_expect_tx(&fullB[slot], kBBytes);
-        ptx::tma_load_3d(sB + slot * kBBytes, &tmB, &fullB[slot], cb * 64, 0, kt);
-      }
-      __syncwarp();
-      if (++slot == kNB) { slot = 0; phase ^= 1; }
-    });
-  } else if (warp == 2) {
-    int slotA = 0, slotB = 0;
+    if (warp == 0) {
+      for_each_step([&](int kt, int ti, int cb) {
+        ptx::mbar_wait(&emptyA[slot], phase ^ 1);
+        if (ptx::elect_one()) {
+          ptx::mbar_expect_tx(&fullA[slot], kSlabBytes);
+          // slab position (0,0) is the input position of output (h0,w0) at tap (0,0)
+          ptx::tma_load_5d(sA + slot * kSlabBytes, &tmA, &fullA[slot], cb * 64, w0 + p.off_w, h0 + p.off_h, ti, b);
+        }
+        __syncwarp();
+        if (++slot == kNA) { slot = 0; phase ^= 1; }
+      });
+    } else if (warp == 1) {
+      for_each_step([&](int kt, int ti, int cb) {
+        ptx::mbar_wait(&emptyB[slot], phase ^ 1);
+        if (ptx::elect_one()) {
+          ptx::mbar_expect_tx(&fullB[slot], kBBytes);
+          ptx::tma_load_3d(sB + slot * kBBytes, &tmB, &fullB[slot], cb * 64, 0, kt);
+        }
+        __syncwarp();
+        if (++slot == kNB) { slot = 0; phase ^= 1; }
+      });
+    }
+    return;
+  }
+
+  // ------------------------------------------------------------- MMA warpgroups: 192 slab positions (3 x 64 rows) each
+  ptx::setmaxnreg_inc<232>();
+  const int half = (threadIdx.x >> 7) - 1;
+  const bool wg_leader = (threadIdx.x & 127) == 0;
+  float acc[kChunks][kNstk / 2];
+  {
+    int slotA = 0, slotB = 0, pendA = -1, pendB = -1;
     uint32_t phaseA = 0, phaseB = 0, accumulate = 0;
-    constexpr uint32_t kDescHi = 64u | (1u << 14) | (2u << 29);
-    constexpr uint32_t kDescLoFlags = 1u << 16;
-    const uint32_t idesc = p.idesc;
     for_each_step([&](int kt, int ti, int cb) {
       ptx::mbar_wait(&fullA[slotA], phaseA);
       ptx::mbar_wait(&fullB[slotB], phaseB);
-      ptx::tc_fence_after();
       const int ch_left = p.Cin - cb * 64;
       const int ksteps = ch_left >= 64 ? 4 : (ch_left + 15) >> 4;
-      const uint32_t a_lo0 = ((ptx::smem_u32(sA + slotA * kSlabBytes) >> 4) & 0x3FFFu) | kDescLoFlags;
-      const uint32_t b_lo0 = ((ptx::smem_u32(sB + slotB * kBBytes) >> 4) & 0x3FFFu) | kDescLoFlags;
-      if (ptx::elect_one()) {
-        for (int s = 0; s < 4; ++s)
-          for (int k = 0; k < ksteps; ++k)
-            ptx::umma_f16_lohi(tmem_base + s * kNstk, a_lo0 + s * (16384u >> 4) + 2 * k, b_lo0 + 2 * k, kDescHi, idesc,
-                               accumulate | static_cast<uint32_t>(k));
-        ptx::umma_commit(&emptyB[slotB]);
-        ptx::umma_commit(&emptyA[slotA]);
-      }
-      __syncwarp();
+      const uint32_t a0 = ptx::smem_u32(sA + slotA * kSlabBytes) + static_cast<uint32_t>(half * kChunks * 64) * 128u;
+      const uint32_t b0 = ptx::smem_u32(sB + slotB * kBBytes);
+      ptx::wgmma_fence();
+#pragma unroll
+      for (int c = 0; c < kChunks; ++c)
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          if (k < ksteps)
+            ptx::Wgmma<DT, kNstk>::run(acc[c], ptx::wgmma_desc_sw128(a0 + c * 8192u + 32u * k), ptx::wgmma_desc_sw128(b0 + 32u * k),
+                                       accumulate | static_cast<uint32_t>(k));
       accumulate = 1;
+      ptx::wgmma_commit();
+      ptx::wgmma_wait<1>();
+      if (wg_leader && pendA >= 0) {
+        ptx::mbar_arrive(&emptyB[pendB]);
+        ptx::mbar_arrive(&emptyA[pendA]);
+      }
+      pendA = slotA;
+      pendB = slotB;
       if (++slotA == kNA) { slotA = 0; phaseA ^= 1; }
       if (++slotB == kNB) { slotB = 0; phaseB ^= 1; }
     });
-    if (ptx::elect_one()) ptx::umma_commit(accFull);
-    __syncwarp();
+    ptx::wgmma_wait<0>();
+#pragma unroll
+    for (int c = 0; c < kChunks; ++c) ptx::fence_regs(acc[c]);
   }
 
-  // ------------------------------------------------------------- epilogue, all 8 warps
-  ptx::mbar_wait(accFull, 0);
-  ptx::tc_fence_after();
-  float* exch = reinterpret_cast<float*>(sA);  // [512 slab positions][xstride]; the A ring is drained
+  // ------------------------------------------------------------- epilogue, both MMA warpgroups
+  ptx::named_bar_sync(1, 256);   // both warpgroups are done reading the A ring
+  float* exch = reinterpret_cast<float*>(sA);  // [384 slab positions][xstride]
   {
-    // phase 1: every slab position writes its 9 x Cout partial sums.  Warp w reads TMEM lanes 32*(w%4)..; the two warps
-    // of a lane quarter split the four sub-tiles.
-    const int q = warp & 3, half = warp >> 2;
-    for (int s = half; s < 4; s += 2) {
-      const int pos = s * 128 + q * 32 + lane;
-      float* dst = exch + static_cast<size_t>(pos) * p.xstride;
-      uint32_t v[32];
-      for (int c0 = 0; c0 < 72; c0 += 32) {
-        ptx::tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(s * kNstk + c0), v);
-        ptx::tmem_ld_wait();
+    // phase 1: every slab position writes its 9 x Cout partial sums (column 8 * tap + channel slot of the accumulator)
+    const int wl = warp & 3;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const int col = c0 + j;          // = tap * 8 + channel slot
-          const int tap = col >> 3, c = col & 7;
-          if (col < 72 && c < p.Cout) dst[tap * p.Cout + c] = __uint_as_float(v[j]);
-        }
+    for (int c = 0; c < kChunks; ++c)
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int pos = (half * kChunks + c) * 64 + wl * 16 + (lane >> 2) + rr * 8;
+        float* dst = exch + static_cast<size_t>(pos) * p.xstride;
+#pragma unroll
+        for (int tap = 0; tap < 9; ++tap)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int ch = 2 * (lane & 3) + e;
+            if (ch < p.Cout) dst[tap * p.Cout + ch] = acc[c][4 * tap + 2 * rr + e];
+          }
       }
-    }
   }
-  ptx::tc_fence_before();
-  __syncthreads();
+  ptx::named_bar_sync(1, 256);
   {
-    // phase 2: outputs gather the nine shifted partials.  512 slab positions over 256 threads.
+    // phase 2: outputs gather the nine shifted partials.  384 slab positions over 256 threads.
     using T = typename E::T;
     T* yb = reinterpret_cast<T*>(p.y) + b * p.ys_b + t * p.ys_t;
-    for (int pos = threadIdx.x; pos < kSlabW * kSlabH; pos += 256) {
+    for (int pos = threadIdx.x - 128; pos < kSlabW * kSlabH; pos += 256) {
       const int r = pos / kSlabW, c = pos % kSlabW;
       if (r >= kOutH || c >= kOutW) continue;   // output (r,c) of the tile reads slab positions (r+kh, c+kw)
       const int ho = h0 + r, wo = w0 + c;
       if (ho >= p.H_out || wo >= p.W_out) continue;
-      float acc[4] = {0.f, 0.f, 0.f, 0.f};
+      float acc4[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
       for (int kh = 0; kh < 3; ++kh)
 #pragma unroll
         for (int kw = 0; kw < 3; ++kw) {
           const float* src = exch + static_cast<size_t>((r + kh) * kSlabW + (c + kw)) * p.xstride + (kh * 3 + kw) * p.Cout;
-          for (int ch = 0; ch < p.Cout; ++ch) acc[ch] += src[ch];
+          for (int ch = 0; ch < p.Cout; ++ch) acc4[ch] += src[ch];
         }
       for (int ch = 0; ch < p.Cout; ++ch) {
-        float a = acc[ch] * p.alpha;
+        float a = acc4[ch] * p.alpha;
         if (p.bias) a += __ldg(p.bias + ch);
         yb[ho * p.ys_h + wo * p.ys_w + ch * p.ys_c] = E::from_f(a);
       }
     }
-  }
-  __syncthreads();
-  if (warp == 3) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, 512);
   }
 }
 
@@ -230,7 +225,6 @@ extern "C" int cvvae_conv3d_stacked(const cvvae_conv_desc* d, void* stream_) {
   p.tiles_w = (p.W_out + kOutW - 1) / kOutW;
   p.tiles_h = (p.H_out + kOutH - 1) / kOutH;
   p.cblocks = (p.Cin + 63) / 64;
-  p.idesc = ptx::umma_idesc_f16(d->dtype == CVVAE_BF16 ? 1 : 0, 128, kNstk);
   p.xstride = (9 * p.Cout) | 1;  // odd stride: conflict-free for consecutive positions
   CUtensorMap tmA, tmB;
   {
@@ -262,7 +256,7 @@ extern "C" int cvvae_conv3d_stacked(const cvvae_conv_desc* d, void* stream_) {
       CVVAE_CUDA(cudaFuncSetAttribute(conv_stk_kernel<DT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
       attr.mark();
     }
-    conv_stk_kernel<DT><<<static_cast<unsigned>(grid), 256, smem, stream>>>(tmA, tmB, p);
+    conv_stk_kernel<DT><<<static_cast<unsigned>(grid), kStkThreads, smem, stream>>>(tmA, tmB, p);
   });
   CVVAE_LAUNCH_CHECK();
   return CVVAE_OK;

@@ -256,8 +256,8 @@ static int fill_view(GnView& v, const cvvae_tensor5* x, const cvvae_tensor5* y, 
 static void pick_grid(GnView& v, int units, dim3& grid) {
   // Positions per CTA depend on the per-unit extent ONLY (not on the batch size, not on the SM count of the device): the
   // fp32 per-thread partial sums of gn_stats_kernel group the same way whether a clip runs alone, in a tile batch or on
-  // another GPU, so tile batching and sharding stay bit-identical at any size.  ~1184 CTAs per unit (8 per SM of a
-  // 148-SM part), at least 256 positions each.
+  // another GPU, so tile batching and sharding stay bit-identical at any size.  ~1184 CTAs per unit (about 9 per SM of a
+  // 132-SM H100), at least 256 positions each.
   constexpr long long kBlocksPerUnit = 1184;
   long long ppb = (v.pix_per_unit + kBlocksPerUnit - 1) / kBlocksPerUnit;
   if (ppb < 256) ppb = 256;

@@ -1,4 +1,4 @@
-"""Encoder / Decoder graphs of CV-VAE executed on the hand-written sm_100a kernels.
+"""Encoder / Decoder graphs of CV-VAE executed on the hand-written sm_90a kernels.
 
 This is the seam the reference crosses with ``self.encoder(tile)`` / ``self.decoder(tile)``
 (models/modeling_vae.py:162,249).  The graphs follow
@@ -131,8 +131,7 @@ class Engine:
         self._stats_next = 0
         self.attn_scratch_bytes = 4 << 30  # cap of the fp32 logits buffer of the batched spatial attention
         # 1x1 shortcuts as extra K steps of conv2 (CVVAE_FUSE_SHORTCUT=0: separate launch + residual add, for A/B runs)
-        # (the experiment knob CVVAE_CONV_WIDE=0 selects a persistent-kernel variant without the shortcut K steps)
-        self.fuse_shortcut = os.environ.get("CVVAE_FUSE_SHORTCUT", "1") != "0" and os.environ.get("CVVAE_CONV_WIDE", "1") != "0"
+        self.fuse_shortcut = os.environ.get("CVVAE_FUSE_SHORTCUT", "1") != "0"
 
     # ------------------------------------------------------------------ shape arithmetic
     def encoded_frames(self, T: int) -> int:

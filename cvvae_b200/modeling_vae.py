@@ -1,4 +1,4 @@
-"""Drop-in ``CVVAEModel`` / ``CVVAESD3Model``: the reference's Python surface over the sm_100a engine.
+"""Drop-in ``CVVAEModel`` / ``CVVAESD3Model``: the reference's Python surface over the sm_90a engine.
 
 Mirrors models/modeling_vae.py of the reference - same constructor keyword arguments and defaults
 (:23-51, :347-381), ``config`` attribute/dict access, ``from_pretrained(path, subfolder=, torch_dtype=)``
@@ -229,7 +229,7 @@ class _CVVAEBase(nn.Module):
                 ops = self._ops_factory()
             else:
                 if p0.device.type != "cuda":
-                    raise RuntimeError("cvvae_b200 runs on CUDA (sm_100a) only: move the model with .cuda(); "
+                    raise RuntimeError("cvvae_b200 runs on CUDA (sm_90a) only: move the model with .cuda(); "
                                        "there is no CPU or PyTorch fallback path")
                 if p0.dtype not in (torch.float16, torch.bfloat16):
                     raise RuntimeError(f"cvvae_b200 computes in float16/bfloat16; model dtype is {p0.dtype} - call .half()")

@@ -65,7 +65,7 @@ def _on_tensor_device(fn):
 
 
 class CudaOps:
-    """The production operator set: every method is one (or two) hand-written sm_100a kernels."""
+    """The production operator set: every method is one (or two) hand-written sm_90a kernels."""
 
     name = "cuda"
 

@@ -1,5 +1,5 @@
 /*
- * cvvae_b200 - C ABI of the B200-native CV-VAE encode()/decode() hot path.
+ * cvvae_b200 - C ABI of the H100-native (sm_90a) CV-VAE encode()/decode() hot path.
  *
  * The reference (AILab-CVC/CV-VAE) is pure Python on PyTorch and has no FFI of its own; the seam this
  * library replaces is the `nn.Module.__call__` operator boundary inside `self.encoder(x)` /
@@ -102,7 +102,7 @@ typedef struct cvvae_conv_desc {
   const void* w2;
 } cvvae_conv_desc;
 
-/* Dispatcher: tcgen05 implicit-GEMM kernel when eligible (x.s_c==1, Cin%8==0, 16B-aligned strides,
+/* Dispatcher: wgmma implicit-GEMM kernel when eligible (x.s_c==1, Cin%8==0, 16B-aligned strides,
  * pad_hw==ZERO), CUDA-core kernel otherwise (e.g. the 3/4-channel network inputs).              */
 int cvvae_conv3d(const cvvae_conv_desc* d, void* stream);
 int cvvae_conv3d_tc(const cvvae_conv_desc* d, void* stream);     /* tensor-core path only */
@@ -196,9 +196,10 @@ const char* cvvae_last_error(void);
 int cvvae_abi_version(void);
 /* Number of kernel launches issued through this library by the calling process (all threads). */
 int64_t cvvae_launch_count(void);
-/* Descriptor self-test used by the GPU test-suite: runs a 128xNx64 UMMA whose A operand starts
- * `row_shift` 128-byte rows into a TMA-written SWIZZLE_128B slab of 320 rows, with the given base_offset field and
- * with consecutive 8-row groups `sbo_rows` (8..16) slab rows apart.  a_rows: [320][64], out: fp32 [128][N].
+/* Descriptor self-test used by the GPU test-suite: runs a 128xNx64 product (two 64-row wgmma chains, N in {64, 128,
+ * 256}) whose A operand starts `row_shift` 128-byte rows into a TMA-written SWIZZLE_128B slab of 320 rows, with the given
+ * base_offset field and with consecutive 8-row groups `sbo_rows` (8..16) slab rows apart.  a_rows: [320][64], out: fp32
+ * [128][N].
  * (Decides how shifted conv taps may address one staged slab.) */
 int cvvae_probe_umma_shift(const void* a_rows, const void* b_rows, float* out, int32_t n, int32_t row_shift,
                            int32_t base_offset_mode, int32_t sbo_rows, void* stream);

@@ -1,4 +1,4 @@
-"""The C-ABI shared library builds for sm_100a, loads without a GPU and exports every symbol include/cvvae_b200.h
+"""The C-ABI shared library builds for sm_90a, loads without a GPU and exports every symbol include/cvvae_b200.h
 declares (no compute calls here)."""
 import ctypes
 import os

@@ -63,7 +63,7 @@ def main():
         tt = t.astype(np.int64)
         tt[:, 7] = (tt[:, 0] & ~np.int64(0xFFFFFFFFFFFF)) | t7
         def d(a, b_):
-            # MMA-issue stamps (columns 2-4) exist only in the CTA that issues (the leader of a pair): use the rows that have both
+            # phase stamps may be missing (untraced CTAs): use the rows that have both
             rows = tt[(t[:, a] > 0) & (t[:, b_] > 0)]
             return float(np.median(rows[:, b_] - rows[:, a])) / 1e3 if len(rows) else None
         # idle gap between consecutive CTAs on the same SM

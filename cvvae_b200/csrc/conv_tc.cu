@@ -230,20 +230,37 @@ __global__ void __launch_bounds__(kThreads, 1)
       if (traced && first && threadIdx.x == 128) trc[3] = ptx::globaltimer_ns();
       first = false;
       const uint32_t b_base = ptx::smem_u32(sB + static_cast<size_t>(slotB) * p.b_bytes);
-      ptx::wgmma_fence();
+      if (nacc_eff == kMaxAcc && ksteps == 4) {
+        // Full tile, nearly all of the work.  Fence, chain and commit sit in one basic block with no branch between the
+        // MMAs, so ptxas issues the chain behind one warpgroup.arrive and closes the group on its last MMA.  Behind a
+        // runtime branch every MMA gets its own arrive and group and the commit becomes a dummy MMA, so wait_group 1
+        // below would wait for all of this group's real MMAs.
+        ptx::wgmma_fence();
 #pragma unroll
-      for (int s = 0; s < kMaxAcc; ++s) {
-        if (s < nacc_eff) {
+        for (int s = 0; s < kMaxAcc; ++s) {
           const uint32_t a_s = a_base + static_cast<uint32_t>(s) * sub_stride;
 #pragma unroll
           for (int k = 0; k < 4; ++k)
-            if (k < ksteps)   // K = 16 per MMA; channels beyond Cin are TMA zero-fill in both operands, skip those MMAs
-              ptx::Wgmma<DT, BN>::run(acc[s], ptx::wgmma_desc_sw128(a_s + 32u * k), ptx::wgmma_desc_sw128(b_base + 32u * k),
-                                      accumulate | static_cast<uint32_t>(k));
+            ptx::Wgmma<DT, BN>::run(acc[s], ptx::wgmma_desc_sw128(a_s + 32u * k), ptx::wgmma_desc_sw128(b_base + 32u * k),
+                                    accumulate | static_cast<uint32_t>(k));
         }
+        ptx::wgmma_commit();
+      } else {
+        ptx::wgmma_fence();
+#pragma unroll
+        for (int s = 0; s < kMaxAcc; ++s) {
+          if (s < nacc_eff) {
+            const uint32_t a_s = a_base + static_cast<uint32_t>(s) * sub_stride;
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+              if (k < ksteps)   // K = 16 per MMA; channels beyond Cin are TMA zero-fill in both operands, skip those MMAs
+                ptx::Wgmma<DT, BN>::run(acc[s], ptx::wgmma_desc_sw128(a_s + 32u * k), ptx::wgmma_desc_sw128(b_base + 32u * k),
+                                        accumulate | static_cast<uint32_t>(k));
+          }
+        }
+        ptx::wgmma_commit();
       }
       accumulate = 1;
-      ptx::wgmma_commit();
       ptx::wgmma_wait<1>();   // the previous group is done reading its operands
       if (wg_leader) {
         if (pendB >= 0) ptx::mbar_arrive(&emptyB[pendB]);
@@ -327,110 +344,156 @@ __global__ void __launch_bounds__(kThreads, 1)
         }
       }
     }
+    // the consumer GroupNorm's statistics of channel pair (cc, cc + 1): reduce over the rows of the warp, add to the bins
+    auto gn_add = [&](float gs0, float gq0, float gs1, float gq1, int cc, bool tok, bool c1ok) {
+      // rows: lanes with the same lane%4 hold the same channels
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      if (tc.n0 + 8 * j >= p.Cout) break;   // warp-uniform
-      const int cg = tc.n0 + 8 * j + cpair;
-      const bool c0ok = cg < p.Cout, c1ok = cg + 1 < p.Cout;
-      // output coordinates (time interleave of Upsample3D folded in); Cout is even with up_time, so cg and cg + 1
-      // land in the same half
-      const int n_il = p.up_time == 2 ? cg / chalf : 0;
-      const int cc = cg - n_il * chalf;
-      const int t_o = p.up_time == 2 ? 2 * tc.t + n_il - 1 : tc.t;
-      const bool tok = t_o >= 0 && c0ok;
-      const long long coff = t_o * p.ys_t + cc * p.ys_c;
-      float b0 = 0.f, b1 = 0.f;
-      if (p.bias && !bias_m) {
-        if (c0ok) b0 = __ldg(p.bias + cg);
-        if (c1ok) b1 = __ldg(p.bias + cg + 1);
+      for (int o = 4; o < 32; o <<= 1) {
+        gs0 += __shfl_xor_sync(0xffffffffu, gs0, o);
+        gq0 += __shfl_xor_sync(0xffffffffu, gq0, o);
+        gs1 += __shfl_xor_sync(0xffffffffu, gs1, o);
+        gq1 += __shfl_xor_sync(0xffffffffu, gq1, o);
       }
-      float gs0 = 0.f, gq0 = 0.f, gs1 = 0.f, gq1 = 0.f;
-#pragma unroll
-      for (int s = 0; s < kMaxAcc; ++s) {
-#pragma unroll
-        for (int rr = 0; rr < 2; ++rr) {
-          if (!rok[s][rr] || !tok) continue;
-          const float bb0 = bias_m ? rbias[s][rr] : b0, bb1 = bias_m ? rbias[s][rr] : b1;
-          float a0 = fmaf(acc[s][4 * j + 2 * rr], p.alpha, bb0);
-          float a1 = fmaf(acc[s][4 * j + 2 * rr + 1], p.alpha, bb1);
-          const long long off = roff[s][rr] + coff;
-          if (out_f32) {
-            // fp32 logits (S = q k^T): no residual, no interleave
-            float* yf = reinterpret_cast<float*>(p.y) + off;
-            if (p.vec2 && c1ok) {
-              *reinterpret_cast<float2*>(yf) = make_float2(a0, a1);
-            } else {
-              yf[0] = a0;
-              if (c1ok) yf[p.ys_c] = a1;
-            }
-            continue;
-          }
-          T* yp = reinterpret_cast<T*>(p.y) + off;
-          const T* rp = p.residual ? reinterpret_cast<const T*>(p.residual) + off : nullptr;
-          if (p.vec2 && c1ok) {
-            if (rp) {
-              const float2 rf = E::to_f2(__ldg(reinterpret_cast<const unsigned int*>(rp)));
-              a0 += rf.x;
-              a1 += rf.y;
-            }
-            const uint32_t o = E::pack2(a0, a1);
-            *reinterpret_cast<uint32_t*>(yp) = o;
-            const float2 of = E::to_f2(o);
-            a0 = of.x;
-            a1 = of.y;
-          } else {
-            if (rp) {
-              a0 += E::to_f(rp[0]);
-              if (c1ok) a1 += E::to_f(rp[p.ys_c]);
-            }
-            const T o0 = E::from_f(a0), o1 = E::from_f(a1);
-            yp[0] = o0;
-            if (c1ok) yp[p.ys_c] = o1;
-            a0 = E::to_f(o0);
-            a1 = E::to_f(o1);
-          }
-          // GroupNorm statistics of the consumer, from the stored (rounded) values
-          gs0 += a0;
-          gq0 = fmaf(a0, a0, gq0);
+      if (p.gn_cpg == 1) {
+        if (lane < 4 && tok) {
+          atomicAdd(&gn_bins[cc * 2], gn_fix(gs0, kGnSumScale));
+          atomicAdd(&gn_bins[cc * 2 + 1], gn_fix(gq0, kGnSqScale));
           if (c1ok) {
-            gs1 += a1;
-            gq1 = fmaf(a1, a1, gq1);
+            atomicAdd(&gn_bins[(cc + 1) * 2], gn_fix(gs1, kGnSumScale));
+            atomicAdd(&gn_bins[(cc + 1) * 2 + 1], gn_fix(gq1, kGnSqScale));
           }
+        }
+      } else {
+        float ts = gs0 + gs1, tq = gq0 + gq1;
+        // channel pairs of one group are neighbouring lanes (lane%4)
+        for (int o = 1; o < (p.gn_cpg >> 1) && o < 4; o <<= 1) {
+          ts += __shfl_xor_sync(0xffffffffu, ts, o);
+          tq += __shfl_xor_sync(0xffffffffu, tq, o);
+        }
+        const int lanes_per_group = min(p.gn_cpg >> 1, 4);
+        // a group's channels never straddle the interleave halves (chalf is a multiple of the group size), so the
+        // first lane of the group has the validity of all of them
+        if (lane < 4 && (lane % lanes_per_group) == 0 && tok) {
+          atomicAdd(&gn_bins[(cc / p.gn_cpg) * 2], gn_fix(ts, kGnSumScale));
+          atomicAdd(&gn_bins[(cc / p.gn_cpg) * 2 + 1], gn_fix(tq, kGnSqScale));
         }
       }
-      if (p.gn_stats) {
-        // rows: lanes with the same lane%4 hold the same channels
+    };
+    // Interior tiles (every row and channel valid, 16-bit output stored as channel-pair words, bias along N) take a
+    // loop without per-element tests.  The general loop's branches kept ptxas from batching the bias / residual loads
+    // and the stores, so its epilogue took a third of a CTA's time.  Same operations in the same order: same bits.
+    const bool interior = nacc_eff == kMaxAcc && tc.n0 + BN <= p.Cout && !out_f32 && p.vec2 && !bias_m &&
+                          (p.flat ? tc.w0 + kMaxAcc * 128 <= p.W_out
+                                  : tc.h0 + kMaxAcc * p.ROWS <= p.H_out && tc.w0 + p.TW <= p.W_out);
+    if (interior) {
 #pragma unroll
-        for (int o = 4; o < 32; o <<= 1) {
-          gs0 += __shfl_xor_sync(0xffffffffu, gs0, o);
-          gq0 += __shfl_xor_sync(0xffffffffu, gq0, o);
-          gs1 += __shfl_xor_sync(0xffffffffu, gs1, o);
-          gq1 += __shfl_xor_sync(0xffffffffu, gq1, o);
-        }
-        if (p.gn_cpg == 1) {
-          if (lane < 4 && tok) {
-            atomicAdd(&gn_bins[cc * 2], gn_fix(gs0, kGnSumScale));
-            atomicAdd(&gn_bins[cc * 2 + 1], gn_fix(gq0, kGnSqScale));
-            if (c1ok) {
-              atomicAdd(&gn_bins[(cc + 1) * 2], gn_fix(gs1, kGnSumScale));
-              atomicAdd(&gn_bins[(cc + 1) * 2 + 1], gn_fix(gq1, kGnSqScale));
+      for (int j = 0; j < BN / 8; ++j) {
+        const int cg = tc.n0 + 8 * j + cpair;
+        const int n_il = p.up_time == 2 ? cg / chalf : 0;
+        const int cc = cg - n_il * chalf;
+        const int t_o = p.up_time == 2 ? 2 * tc.t + n_il - 1 : tc.t;
+        const bool tok = t_o >= 0;
+        const long long coff = t_o * p.ys_t + cc * p.ys_c;
+        const float b0 = p.bias ? __ldg(p.bias + cg) : 0.f, b1 = p.bias ? __ldg(p.bias + cg + 1) : 0.f;
+        float gs0 = 0.f, gq0 = 0.f, gs1 = 0.f, gq1 = 0.f;
+        if (tok) {
+#pragma unroll
+          for (int s = 0; s < kMaxAcc; ++s) {
+#pragma unroll
+            for (int rr = 0; rr < 2; ++rr) {
+              float a0 = fmaf(acc[s][4 * j + 2 * rr], p.alpha, b0);
+              float a1 = fmaf(acc[s][4 * j + 2 * rr + 1], p.alpha, b1);
+              const long long off = roff[s][rr] + coff;
+              if (p.residual) {
+                const float2 rf = E::to_f2(__ldg(reinterpret_cast<const unsigned int*>(reinterpret_cast<const T*>(p.residual) + off)));
+                a0 += rf.x;
+                a1 += rf.y;
+              }
+              const uint32_t o = E::pack2(a0, a1);
+              *reinterpret_cast<uint32_t*>(reinterpret_cast<T*>(p.y) + off) = o;
+              const float2 of = E::to_f2(o);
+              gs0 += of.x;
+              gq0 = fmaf(of.x, of.x, gq0);
+              gs1 += of.y;
+              gq1 = fmaf(of.y, of.y, gq1);
             }
           }
-        } else {
-          float ts = gs0 + gs1, tq = gq0 + gq1;
-          // channel pairs of one group are neighbouring lanes (lane%4)
-          for (int o = 1; o < (p.gn_cpg >> 1) && o < 4; o <<= 1) {
-            ts += __shfl_xor_sync(0xffffffffu, ts, o);
-            tq += __shfl_xor_sync(0xffffffffu, tq, o);
-          }
-          const int lanes_per_group = min(p.gn_cpg >> 1, 4);
-          // a group's channels never straddle the interleave halves (chalf is a multiple of the group size), so the
-          // first lane of the group has the validity of all of them
-          if (lane < 4 && (lane % lanes_per_group) == 0 && tok) {
-            atomicAdd(&gn_bins[(cc / p.gn_cpg) * 2], gn_fix(ts, kGnSumScale));
-            atomicAdd(&gn_bins[(cc / p.gn_cpg) * 2 + 1], gn_fix(tq, kGnSqScale));
+        }
+        if (p.gn_stats) gn_add(gs0, gq0, gs1, gq1, cc, tok, true);
+      }
+    } else {
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        if (tc.n0 + 8 * j >= p.Cout) break;   // warp-uniform
+        const int cg = tc.n0 + 8 * j + cpair;
+        const bool c0ok = cg < p.Cout, c1ok = cg + 1 < p.Cout;
+        // output coordinates (time interleave of Upsample3D folded in); Cout is even with up_time, so cg and cg + 1
+        // land in the same half
+        const int n_il = p.up_time == 2 ? cg / chalf : 0;
+        const int cc = cg - n_il * chalf;
+        const int t_o = p.up_time == 2 ? 2 * tc.t + n_il - 1 : tc.t;
+        const bool tok = t_o >= 0 && c0ok;
+        const long long coff = t_o * p.ys_t + cc * p.ys_c;
+        float b0 = 0.f, b1 = 0.f;
+        if (p.bias && !bias_m) {
+          if (c0ok) b0 = __ldg(p.bias + cg);
+          if (c1ok) b1 = __ldg(p.bias + cg + 1);
+        }
+        float gs0 = 0.f, gq0 = 0.f, gs1 = 0.f, gq1 = 0.f;
+#pragma unroll
+        for (int s = 0; s < kMaxAcc; ++s) {
+#pragma unroll
+          for (int rr = 0; rr < 2; ++rr) {
+            if (!rok[s][rr] || !tok) continue;
+            const float bb0 = bias_m ? rbias[s][rr] : b0, bb1 = bias_m ? rbias[s][rr] : b1;
+            float a0 = fmaf(acc[s][4 * j + 2 * rr], p.alpha, bb0);
+            float a1 = fmaf(acc[s][4 * j + 2 * rr + 1], p.alpha, bb1);
+            const long long off = roff[s][rr] + coff;
+            if (out_f32) {
+              // fp32 logits (S = q k^T): no residual, no interleave
+              float* yf = reinterpret_cast<float*>(p.y) + off;
+              if (p.vec2 && c1ok) {
+                *reinterpret_cast<float2*>(yf) = make_float2(a0, a1);
+              } else {
+                yf[0] = a0;
+                if (c1ok) yf[p.ys_c] = a1;
+              }
+              continue;
+            }
+            T* yp = reinterpret_cast<T*>(p.y) + off;
+            const T* rp = p.residual ? reinterpret_cast<const T*>(p.residual) + off : nullptr;
+            if (p.vec2 && c1ok) {
+              if (rp) {
+                const float2 rf = E::to_f2(__ldg(reinterpret_cast<const unsigned int*>(rp)));
+                a0 += rf.x;
+                a1 += rf.y;
+              }
+              const uint32_t o = E::pack2(a0, a1);
+              *reinterpret_cast<uint32_t*>(yp) = o;
+              const float2 of = E::to_f2(o);
+              a0 = of.x;
+              a1 = of.y;
+            } else {
+              if (rp) {
+                a0 += E::to_f(rp[0]);
+                if (c1ok) a1 += E::to_f(rp[p.ys_c]);
+              }
+              const T o0 = E::from_f(a0), o1 = E::from_f(a1);
+              yp[0] = o0;
+              if (c1ok) yp[p.ys_c] = o1;
+              a0 = E::to_f(o0);
+              a1 = E::to_f(o1);
+            }
+            // GroupNorm statistics of the consumer, from the stored (rounded) values
+            gs0 += a0;
+            gq0 = fmaf(a0, a0, gq0);
+            if (c1ok) {
+              gs1 += a1;
+              gq1 = fmaf(a1, a1, gq1);
+            }
           }
         }
+        if (p.gn_stats) gn_add(gs0, gq0, gs1, gq1, cc, tok, c1ok);
       }
     }
   }

@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Per-layer microbenchmark of the tensor-core convolution on the distinct conv problems of one
-17x576x576 tile (SURVEY.md section 3.6).  Prints one JSON line per problem: ms, TFLOP/s, fraction of the measured
-bf16 peak.  L2 is flushed between timed launches (256 MB memset) and each timing is the median of `reps`.
+17x576x576 tile (SURVEY.md section 3.6).  Prints one JSON line per problem: ms, TFLOP/s, fraction of the peak bench.py
+uses (MEASURED_PEAKS.json when present, else the H100 SXM data-sheet 989 TFLOP/s).  L2 is flushed between timed
+launches (256 MB memset) and each timing is the median of `reps`.
 
     python tools/bench_conv.py [--reps 5] [--only substring] [--scale 1.0]
 """
@@ -14,6 +15,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+import bench  # noqa: E402  (the same peak source as the benchmark)
 from cvvae_b200._lib import PAD_REPLICATE, PAD_ZERO  # noqa: E402
 from cvvae_b200.ops import CudaOps  # noqa: E402
 
@@ -47,10 +49,7 @@ def main():
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--only", default="")
     args = ap.parse_args()
-    peak = 1452.6
-    pk = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(pk):
-        peak = json.load(open(pk)).get("bf16_tflops", peak)
+    peak, _ = bench.peaks()
     ops = CudaOps()
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
     dt = torch.float16

@@ -62,12 +62,16 @@ _SIGNATURES = {
     "cvvae_video_resize_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                         C.c_int32, C.c_void_p]),
     "cvvae_conv_tc_set_trace": (C.c_int, [C.c_void_p, C.c_int32]),
+    "cvvae_conv_tc_plan": (C.c_int, [C.POINTER(ConvDesc), C.POINTER(C.c_int32), C.c_int32]),
     "cvvae_last_error": (C.c_char_p, []),
     "cvvae_abi_version": (C.c_int, []),
     "cvvae_launch_count": (C.c_int64, []),
     "cvvae_probe_umma_shift": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
 }
 EXPORTS = tuple(_SIGNATURES)
+# the values cvvae_conv_tc_plan() writes, in order
+CONV_TC_PLAN_FIELDS = ("eligible", "N_cta", "NACC", "TW", "ROWS", "TH", "tiles_w", "tiles_h", "n_tiles_n", "flat", "NA", "NB",
+                       "grid", "vec2")
 
 _lib = None
 

@@ -624,7 +624,10 @@ static int launch_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUten
   return CVVAE_OK;
 }
 
-int conv_tc_launch(const cvvae_conv_desc* d, cudaStream_t stream) {
+// The launch plan of a descriptor: geometry, epilogue pointers and strides, tiling (N_cta, NACC, TW / TH, tile counts),
+// operand ring depths, dynamic shared memory and grid.  conv_tc_launch runs exactly this plan and cvvae_conv_tc_plan
+// reports it, so a test can check which plan it ran.  The fused shortcut, GroupNorm and trace fields are the launch's.
+static int conv_tc_plan(const cvvae_conv_desc* d, ConvTcParams& p, size_t& smem, long long& grid) {
   const char* why = nullptr;
   if (!conv_tc_eligible(d, &why)) {
     set_error("cvvae_conv3d_tc: not eligible: %s", why);
@@ -632,7 +635,7 @@ int conv_tc_launch(const cvvae_conv_desc* d, cudaStream_t stream) {
   }
   const cvvae_tensor5& x = d->x;
   const cvvae_tensor5& y = d->y;
-  ConvTcParams p{};
+  p = ConvTcParams{};
   p.B = x.B;
   p.T_in = x.T;
   p.Cin = x.C;
@@ -652,8 +655,6 @@ int conv_tc_launch(const cvvae_conv_desc* d, cudaStream_t stream) {
   p.y = y.ptr;
   p.ys_b = y.s_b; p.ys_t = y.s_t; p.ys_h = y.s_h; p.ys_w = y.s_w; p.ys_c = y.s_c;
   p.yC = y.C;
-  p.trace = g_trace_buf;
-  p.trace_n = g_trace_n;
   if (d->flags & CVVAE_CONV_X_SHARED) CVVAE_CHECK_ARG(x.B == 1, "conv: CVVAE_CONV_X_SHARED needs x.B == 1");
   else CVVAE_CHECK_ARG(y.B == x.B, "conv: batch mismatch");
   if (d->flags & CVVAE_CONV_W_PER_BATCH)
@@ -735,7 +736,24 @@ int conv_tc_launch(const cvvae_conv_desc* d, cudaStream_t stream) {
   while (NB < 8 && static_cast<size_t>(NB + 1) * p.b_bytes + static_cast<size_t>(NA) * p.slab_stride <= budget) ++NB;
   p.NA = NA;
   p.NB = NB;
-  const size_t smem = 1024 + static_cast<size_t>(NA) * p.slab_stride + static_cast<size_t>(NB) * p.b_bytes + kBarBytes;
+  smem = 1024 + static_cast<size_t>(NA) * p.slab_stride + static_cast<size_t>(NB) * p.b_bytes + kBarBytes;
+
+  grid = 1ll * p.n_tiles_n * p.T_out * p.tiles_w * p.tiles_h * p.B;
+  CVVAE_CHECK_ARG(grid > 0 && grid < (1ll << 31), "conv_tc: grid size %lld out of range", grid);
+  return CVVAE_OK;
+}
+
+int conv_tc_launch(const cvvae_conv_desc* d, cudaStream_t stream) {
+  ConvTcParams p;
+  size_t smem = 0;
+  long long grid = 0;
+  const int prc = conv_tc_plan(d, p, smem, grid);
+  if (prc != CVVAE_OK) return prc;
+  const cvvae_tensor5& x = d->x;
+  const cvvae_tensor5& y = d->y;
+  const int N_cta = p.N_cta;
+  p.trace = g_trace_buf;
+  p.trace_n = g_trace_n;
 
   // ---- tensor maps
   CUtensorMap tmA, tmB;
@@ -814,8 +832,6 @@ int conv_tc_launch(const cvvae_conv_desc* d, cudaStream_t stream) {
     p.gn_cpg = cpg;
   }
 
-  const long long grid = 1ll * p.n_tiles_n * p.T_out * p.tiles_w * p.tiles_h * p.B;
-  CVVAE_CHECK_ARG(grid > 0 && grid < (1ll << 31), "conv_tc: grid size %lld out of range", grid);
   int rc = CVVAE_OK;
   CVVAE_DISPATCH_DTYPE(d->dtype, {
     if (N_cta == 256) rc = launch_bn<DT, 256>(tmA, tmB, tmA2, tmB2, p, static_cast<unsigned>(grid), smem, stream);
@@ -827,11 +843,43 @@ int conv_tc_launch(const cvvae_conv_desc* d, cudaStream_t stream) {
   return CVVAE_OK;
 }
 
+static int conv_tc_plan_query(const cvvae_conv_desc* d, int32_t* out, int32_t n) {
+  ConvTcParams p;
+  size_t smem = 0;
+  long long grid = 0;
+  const int rc = conv_tc_plan(d, p, smem, grid);
+  if (rc != CVVAE_OK && rc != CVVAE_E_UNSUPPORTED) return rc;
+  const bool ok = rc == CVVAE_OK;
+  const int32_t v[] = {ok ? 1 : 0,
+                       ok ? p.N_cta : 0,
+                       ok ? p.NACC : 0,
+                       ok ? p.TW : 0,
+                       ok ? p.ROWS : 0,
+                       ok ? p.TH : 0,
+                       ok ? p.tiles_w : 0,
+                       ok ? p.tiles_h : 0,
+                       ok ? p.n_tiles_n : 0,
+                       ok ? p.flat : 0,
+                       ok ? p.NA : 0,
+                       ok ? p.NB : 0,
+                       ok ? static_cast<int32_t>(grid) : 0,
+                       ok ? p.vec2 : 0};
+  constexpr int32_t kFields = static_cast<int32_t>(sizeof(v) / sizeof(v[0]));
+  for (int32_t i = 0; i < n && i < kFields; ++i) out[i] = v[i];
+  return kFields;
+}
+
 }  // namespace cvvae
 
 extern "C" int cvvae_conv_tc_set_trace(void* device_buf, int32_t n_ctas) {
   cvvae::conv_tc_set_trace(static_cast<unsigned long long*>(device_buf), device_buf ? n_ctas : 0);
   return CVVAE_OK;
+}
+
+extern "C" int cvvae_conv_tc_plan(const cvvae_conv_desc* d, int32_t* out, int32_t n) {
+  CVVAE_CHECK_ARG(d && cvvae::tensor_ok(&d->x) && cvvae::tensor_ok(&d->y) && d->w && (out || n <= 0),
+                  "cvvae_conv_tc_plan: null argument");
+  return cvvae::conv_tc_plan_query(d, out, n);
 }
 
 extern "C" int cvvae_conv3d_tc(const cvvae_conv_desc* d, void* stream) {

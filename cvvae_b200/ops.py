@@ -128,46 +128,15 @@ class CudaOps:
         ``x_shared`` - x has batch 1 and is the left operand of every batch item.
         Fused 1x1 shortcut: ``sc_x`` [B,T,H,W,C2] (the output's extents) times ``sc_w`` [Cout, C2] is accumulated into the
         same fp32 accumulators as the taps (``bias`` then carries the sum of both biases)."""
+        d = self._conv_desc(x, w, bias, kernel=kernel, stride=stride, offset=offset, pad_t=pad_t, pad_hw=pad_hw,
+                            up_time=up_time, residual=residual, alpha=alpha, out=out, out_f32=out_f32,
+                            bias_along_m=bias_along_m, w_ld=w_ld, cout=cout, gn_stats=gn_stats, gn_groups=gn_groups,
+                            w_per_batch=w_per_batch, x_shared=x_shared, sc_x=sc_x, sc_w=sc_w)
         B, T, H, W, Ci = x.shape
         if x_shared:
             B = out.shape[0]
         kt, kh, kw = kernel
-        st, sh, sw = stride
-        ot, oh, ow = offset
-        Co = cout if cout is not None else w.shape[1]
-        assert w.shape[0] == (out.shape[0] if w_per_batch else kt * kh * kw), (w.shape, kernel)
-        if out is None:
-            # PyTorch conv arithmetic with the padding implied by the offsets: out = floor((in + pad - k)/s) + 1,
-            # where the engine always passes offsets so that the reference's output extents result.
-            raise ValueError("conv(): the caller provides `out` (the engine knows the reference's output extents)")
-        d = L.ConvDesc()
-        d.x = _t5(x)
-        d.y = _t5(out)
-        d.w = w.data_ptr()
-        d.w_ld = w_ld
-        d.bias = _ptr(bias)
-        d.residual = _ptr(residual)
-        d.Cout = Co
-        d.KT, d.KH, d.KW = kt, kh, kw
-        d.st, d.sh, d.sw = st, sh, sw
-        d.off_t, d.off_h, d.off_w = ot, oh, ow
-        d.pad_t, d.pad_hw = pad_t, pad_hw
-        d.up_time = up_time
-        d.dtype = dtype_code(x.dtype)
-        d.flags = ((L.CONV_BIAS_ALONG_M if bias_along_m else 0) | (L.CONV_OUT_F32 if out_f32 else 0) |
-                   (L.CONV_W_PER_BATCH if w_per_batch else 0) | (L.CONV_X_SHARED if x_shared else 0))
-        d.alpha = alpha
-        if gn_stats is not None:  # int64 fixed point [B, groups, 2], zeroed by the caller; the epilogue accumulates into it
-            assert gn_stats.dtype == torch.int64 and gn_stats.is_contiguous()
-            d.gn_stats = gn_stats.data_ptr()
-            d.gn_groups = gn_groups
-        if residual is not None:
-            assert residual.shape == out.shape and residual.stride() == out.stride(), "residual must share y's geometry"
-        if sc_w is not None:
-            assert sc_x is not None and tuple(sc_x.shape[:4]) == tuple(out.shape[:4]) and tuple(sc_w.shape) == (Co, sc_x.shape[4])
-            assert sc_w.is_contiguous() and sc_w.dtype == x.dtype
-            d.x2 = _t5(sc_x)
-            d.w2 = sc_w.data_ptr()
+        Co = d.Cout
         fn = {None: self.lib.cvvae_conv3d, "tc": self.lib.cvvae_conv3d_tc, "direct": self.lib.cvvae_conv3d_direct}[force]
         if self.profile is None:
             L.check(fn(C.byref(d), _stream(x)), "cvvae_conv3d")
@@ -196,6 +165,62 @@ class CudaOps:
         e_ev.record()
         self.profile["events"][path].append((s_ev, e_ev))
         return out
+
+    @_on_tensor_device
+    def conv_tc_plan(self, x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], **kw) -> dict:
+        """The tile plan ``conv(..., force="tc")`` launches for the same arguments on the current device
+        ({name: value} over ``_lib.CONV_TC_PLAN_FIELDS``; ``eligible`` 0 when the tensor-core path refuses them).
+        Launches nothing."""
+        d = self._conv_desc(x, w, bias, **kw)
+        n = len(L.CONV_TC_PLAN_FIELDS)
+        vals = (C.c_int32 * n)()
+        rc = self.lib.cvvae_conv_tc_plan(C.byref(d), vals, n)
+        if rc < 0:
+            L.check(rc, "cvvae_conv_tc_plan")
+        return dict(zip(L.CONV_TC_PLAN_FIELDS, list(vals)))
+
+    @staticmethod
+    def _conv_desc(x, w, bias, *, kernel=(1, 1, 1), stride=(1, 1, 1), offset=(0, 0, 0), pad_t=L.PAD_ZERO, pad_hw=L.PAD_ZERO,
+                   up_time=1, residual=None, alpha=1.0, out=None, out_f32=False, bias_along_m=False, w_ld=0, cout=None,
+                   gn_stats=None, gn_groups=32, w_per_batch=False, x_shared=False, sc_x=None, sc_w=None) -> L.ConvDesc:
+        kt, kh, kw = kernel
+        st, sh, sw = stride
+        ot, oh, ow = offset
+        Co = cout if cout is not None else w.shape[1]
+        if out is None:
+            # PyTorch conv arithmetic with the padding implied by the offsets: out = floor((in + pad - k)/s) + 1,
+            # where the engine always passes offsets so that the reference's output extents result.
+            raise ValueError("conv(): the caller provides `out` (the engine knows the reference's output extents)")
+        assert w.shape[0] == (out.shape[0] if w_per_batch else kt * kh * kw), (w.shape, kernel)
+        d = L.ConvDesc()
+        d.x = _t5(x)
+        d.y = _t5(out)
+        d.w = w.data_ptr()
+        d.w_ld = w_ld
+        d.bias = _ptr(bias)
+        d.residual = _ptr(residual)
+        d.Cout = Co
+        d.KT, d.KH, d.KW = kt, kh, kw
+        d.st, d.sh, d.sw = st, sh, sw
+        d.off_t, d.off_h, d.off_w = ot, oh, ow
+        d.pad_t, d.pad_hw = pad_t, pad_hw
+        d.up_time = up_time
+        d.dtype = dtype_code(x.dtype)
+        d.flags = ((L.CONV_BIAS_ALONG_M if bias_along_m else 0) | (L.CONV_OUT_F32 if out_f32 else 0) |
+                   (L.CONV_W_PER_BATCH if w_per_batch else 0) | (L.CONV_X_SHARED if x_shared else 0))
+        d.alpha = alpha
+        if gn_stats is not None:  # int64 fixed point [B, groups, 2], zeroed by the caller; the epilogue accumulates into it
+            assert gn_stats.dtype == torch.int64 and gn_stats.is_contiguous()
+            d.gn_stats = gn_stats.data_ptr()
+            d.gn_groups = gn_groups
+        if residual is not None:
+            assert residual.shape == out.shape and residual.stride() == out.stride(), "residual must share y's geometry"
+        if sc_w is not None:
+            assert sc_x is not None and tuple(sc_x.shape[:4]) == tuple(out.shape[:4]) and tuple(sc_w.shape) == (Co, sc_x.shape[4])
+            assert sc_w.is_contiguous() and sc_w.dtype == x.dtype
+            d.x2 = _t5(sc_x)
+            d.w2 = sc_w.data_ptr()
+        return d
 
     @_on_tensor_device
     def conv_stacked(self, x: torch.Tensor, w_stk: torch.Tensor, bias: Optional[torch.Tensor], *, kt: int, cout: int,

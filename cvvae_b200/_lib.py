@@ -9,10 +9,10 @@ import os
 
 from ._build import LIBPATH
 
-F16, BF16 = 0, 1
+F16, BF16, F32 = 0, 1, 2
 PAD_ZERO, PAD_REPLICATE = 0, 1
 CONV_BIAS_ALONG_M, CONV_FORCE_DIRECT, CONV_OUT_F32, CONV_W_PER_BATCH, CONV_X_SHARED = 1, 2, 4, 8, 16
-ABI_VERSION = 2
+ABI_VERSION = 3
 
 
 class Tensor5(C.Structure):

@@ -1,13 +1,15 @@
 // Attention pieces that are not GEMMs.  The GEMMs of the attention blocks (q/k/v/proj 1x1 convs, S = q k^T,
 // O = P v) run on the tcgen05 convolution kernel as 1x1x1 "flat" problems (see engine.py); here:
-//   * row softmax  fp32 logits -> 16-bit probabilities     (models/vae_models.py:456,518,607)
+//   * row softmax  fp32 logits -> probabilities in the activation dtype (models/vae_models.py:456,518,607); in fp32
+//     storage they feed only the O = P v product and are stored rounded to the nearest TF32 value
 //   * temporal attention over the latent frames of one chunk (models/vae_models.py:573-587)
 #include "common.cuh"
 
 namespace cvvae {
 
-// One CTA per row.  The row is cached in shared memory (one HBM read of the fp32 logits, one 16-bit write); 128-bit loads
-// and 64-bit stores when the row start and leading dimensions allow (the engine's buffers always do), scalar otherwise.
+// One CTA per row.  The row is cached in shared memory (one HBM read of the fp32 logits, one write); 128-bit loads
+// and 64-bit (16-bit storage) / 128-bit (fp32) stores when the row start and leading dimensions allow (the engine's buffers
+// always do), scalar otherwise.
 template <int DT>
 __global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restrict__ s, long long ld_s, void* p_,
                                                            long long ld_p, int cols, int vec) {
@@ -60,12 +62,17 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restri
   const float inv = 1.0f / sum;
   for (int c = threadIdx.x; c < cols4; c += blockDim.x) {
     const float4 v = reinterpret_cast<float4*>(row)[c];
-    uint2 o;
-    o.x = E::pack2(v.x * inv, v.y * inv);
-    o.y = E::pack2(v.z * inv, v.w * inv);
-    reinterpret_cast<uint2*>(pp)[c] = o;
+    if constexpr (DT == CVVAE_F32) {
+      reinterpret_cast<float4*>(pp)[c] =
+          make_float4(E::mma_in(v.x * inv), E::mma_in(v.y * inv), E::mma_in(v.z * inv), E::mma_in(v.w * inv));
+    } else {
+      uint2 o;
+      o.x = E::pack2(v.x * inv, v.y * inv);
+      o.y = E::pack2(v.z * inv, v.w * inv);
+      reinterpret_cast<uint2*>(pp)[c] = o;
+    }
   }
-  for (int c = cols4 * 4 + threadIdx.x; c < cols; c += blockDim.x) pp[c] = E::from_f(row[c] * inv);
+  for (int c = cols4 * 4 + threadIdx.x; c < cols; c += blockDim.x) pp[c] = E::from_f(E::mma_in(row[c] * inv));
 }
 
 struct TAttnParams {
@@ -102,15 +109,11 @@ __global__ void __launch_bounds__(128) attn_temporal_kernel(const TAttnParams p)
     for (int j = 0; j < p.T; ++j) {
       float d = 0.f;
       for (int vi = lane; vi < vecs; vi += 32) {
-        const uint4 a = __ldg(reinterpret_cast<const uint4*>(qb + i * p.qs[1]) + vi);
-        const uint4 c = __ldg(reinterpret_cast<const uint4*>(kb + j * p.ks[1]) + vi);
-        const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, cw[4] = {c.x, c.y, c.z, c.w};
+        float fa[8], fc[8];
+        unpack8<DT>(ld8<DT>(qb + i * p.qs[1] + vi * 8), fa);
+        unpack8<DT>(ld8<DT>(kb + j * p.ks[1] + vi * 8), fc);
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const float2 fa = E::to_f2(aw[e]), fc = E::to_f2(cw[e]);
-          d = fmaf(fa.x, fc.x, d);
-          d = fmaf(fa.y, fc.y, d);
-        }
+        for (int e = 0; e < 8; ++e) d = fmaf(fa[e], fc[e], d);
       }
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
@@ -129,22 +132,13 @@ __global__ void __launch_bounds__(128) attn_temporal_kernel(const TAttnParams p)
 #pragma unroll
       for (int e = 0; e < 8; ++e) acc[e] = 0.f;
       for (int j = 0; j < p.T; ++j) {
-        const uint4 c = __ldg(reinterpret_cast<const uint4*>(vb + j * p.vs[1]) + vi);
-        const uint32_t cw[4] = {c.x, c.y, c.z, c.w};
+        float fc[8];
+        unpack8<DT>(ld8<DT>(vb + j * p.vs[1] + vi * 8), fc);
         const float pj = sc[j] * inv;
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const float2 fc = E::to_f2(cw[e]);
-          acc[2 * e] = fmaf(pj, fc.x, acc[2 * e]);
-          acc[2 * e + 1] = fmaf(pj, fc.y, acc[2 * e + 1]);
-        }
+        for (int e = 0; e < 8; ++e) acc[e] = fmaf(pj, fc[e], acc[e]);
       }
-      uint4 ov;
-      ov.x = E::pack2(acc[0], acc[1]);
-      ov.y = E::pack2(acc[2], acc[3]);
-      ov.z = E::pack2(acc[4], acc[5]);
-      ov.w = E::pack2(acc[6], acc[7]);
-      reinterpret_cast<uint4*>(ob + i * p.os[1])[vi] = ov;
+      st8<DT>(ob + i * p.os[1] + vi * 8, pack8<DT>(acc));
     }
   }
 }
@@ -167,7 +161,7 @@ extern "C" int cvvae_softmax_rows(const float* s, int64_t ld_s, void* p, int64_t
       attr.mark();
     }
     const int vec = (ld_s % 4 == 0) && (ld_p % 4 == 0) && (reinterpret_cast<uintptr_t>(s) % 16 == 0) &&
-                    (reinterpret_cast<uintptr_t>(p) % 8 == 0);
+                    (reinterpret_cast<uintptr_t>(p) % (4 * sizeof(typename Elem<DT>::T)) == 0);
     softmax_rows_kernel<DT><<<static_cast<unsigned>(rows), 256, smem, stream>>>(s, ld_s, p, ld_p, cols, vec);
   });
   CVVAE_LAUNCH_CHECK();

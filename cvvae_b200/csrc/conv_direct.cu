@@ -135,7 +135,8 @@ int conv_direct_launch(const cvvae_conv_desc* d, cudaStream_t stream) {
   return CVVAE_OK;
 }
 
-// [Cout][Cin][taps] -> [taps][Cout][Cin]
+// [Cout][Cin][taps] -> [taps][Cout][Cin]; fp32 weights are stored rounded to the nearest TF32 value, the precision the
+// tensor cores multiply them in
 template <int DT>
 __global__ void pack_weight_kernel(const typename Elem<DT>::T* __restrict__ src, typename Elem<DT>::T* __restrict__ dst,
                                    int Cout, int Cin, int taps) {
@@ -146,7 +147,9 @@ __global__ void pack_weight_kernel(const typename Elem<DT>::T* __restrict__ src,
     const long long r = i / Cin;
     const int co = static_cast<int>(r % Cout);
     const int tap = static_cast<int>(r / Cout);
-    dst[i] = src[(static_cast<long long>(co) * Cin + ci) * taps + tap];
+    const typename Elem<DT>::T v = src[(static_cast<long long>(co) * Cin + ci) * taps + tap];
+    if constexpr (DT == CVVAE_F32) dst[i] = tf32_rn(v);
+    else dst[i] = v;
   }
 }
 

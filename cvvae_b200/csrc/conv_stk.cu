@@ -250,7 +250,7 @@ extern "C" int cvvae_conv3d_stacked(const cvvae_conv_desc* d, void* stream_) {
   CVVAE_CHECK_ARG(grid > 0 && grid < (1ll << 31), "cvvae_conv3d_stacked: grid out of range");
   const size_t smem = 1024 + kNA * kSlabBytes + kNB * kBBytes + 256;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  CVVAE_DISPATCH_DTYPE(d->dtype, {
+  CVVAE_DISPATCH_DTYPE16(d->dtype, "cvvae_conv3d_stacked", {
     static PerDeviceOnce attr;
     if (attr.need()) {
       CVVAE_CUDA(cudaFuncSetAttribute(conv_stk_kernel<DT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

@@ -6,16 +6,17 @@
 // every 128-position sub-tile and keeps NACC accumulators of 64 x BN fp32 (NACC * BN = 256: 128 registers per thread),
 // so every weight tile staged in shared memory feeds 2 * NACC MMAs, and every activation slab feeds all KH row-taps:
 //
-//   A slab  (one per kt, kw, 64-channel block): the (TH+KH-1) x TW input window, shifted by kw, loaded by ONE 5-D TMA
-//           box into a SWIZZLE_128B buffer [row][w][64 ch].  Because the slab pitch is exactly TW positions (a multiple
+//   A slab  (one per kt, kw, channel block): the (TH+KH-1) x TW input window, shifted by kw, loaded by ONE 5-D TMA
+//           box into a SWIZZLE_128B buffer [row][w][128 B of channels: 64 in 16-bit storage, 32 in fp32].  Because the slab pitch is exactly TW positions (a multiple
 //           of 8 -> 1024 B), the A operand of row-tap kh / sub-tile s / half h is the same buffer at byte offset
 //           ((s*ROWS + kh) * TW + 64h) * 128: a 1024-B aligned wgmma descriptor, no copy.  Zero padding in H/W is TMA
 //           out-of-bounds fill; time padding is a coordinate clamp (replicate) or a skipped tap (zeros).  Strided
 //           (down-sampling) convs use TMA element strides.
-//   B tile  (one per tap, 64-channel block): [BN][64] slice of the packed weights [tap][Cout][Cin].
+//   B tile  (one per tap, channel block): [BN][128 B] slice of the packed weights [tap][Cout][Cin].
+// A channel block is fed by 4 MMAs of 32 B each: K = 16 (f16 / bf16) or K = 8 (fp32 storage, TF32 products).
 //
 // Warpgroups (384 threads): 0 = producers (warp 0 slabs, warp 1 weights; registers handed to the MMA warpgroups),
-// 1 and 2 = MMA issue + epilogue (registers -> bias/alpha/residual -> 16-bit stores, with the time-interleave scatter of
+// 1 and 2 = MMA issue + epilogue (registers -> bias/alpha/residual -> stores in the activation dtype, with the time-interleave scatter of
 // Upsample3D folded into the store address, and the consumer GroupNorm's statistics).
 //
 // Replaces cuDNN behind CausalConv3d / nn.Conv3d / Conv2dWithExtraDim / Downsample3D / Upsample3D
@@ -46,7 +47,7 @@ struct ConvTcParams {
   int yC, vec2;        // vec2: channel pairs may be stored (and residual pairs loaded) as one 32-bit / 64-bit word
   int64_t* gn_stats;   // fused GroupNorm statistics of y
   int gn_groups, gn_cpg;
-  // fused 1x1 shortcut (ResnetBlock3D nin_shortcut / conv_shortcut as extra K steps of conv2): cblocks2 64-channel blocks
+  // fused 1x1 shortcut (ResnetBlock3D nin_shortcut / conv_shortcut as extra K steps of conv2): cblocks2 channel blocks
   // of a second input tensor (same positions as the output) times a [Cout][Cin2] matrix, accumulated after the taps
   int Cin2, cblocks2;
   unsigned long long* trace;  // optional [trace_n][8] globaltimer stamps per CTA (diagnostics)
@@ -101,6 +102,10 @@ __global__ void __launch_bounds__(kThreads, 1)
   constexpr int kMaxAcc = 256 / BN;   // 128-position sub-tiles per CTA at most
   constexpr int kR = BN / 2;          // accumulator registers per thread per sub-tile
   using E = Elem<DT>;
+  // channels per 128-byte operand row (one channel block: 64 in 16-bit storage, 32 in fp32) and K per MMA (a quarter)
+  constexpr int kCB = 128 / static_cast<int>(sizeof(typename E::T));
+  constexpr int kKmma = kCB / 4;
+  constexpr int kKshift = kKmma == 16 ? 4 : 3;   // log2(kKmma)
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;
@@ -166,21 +171,21 @@ __global__ void __launch_bounds__(kThreads, 1)
           if (p.flat) {
             ptx::mbar_expect_tx(&fullA[slot], static_cast<uint32_t>(nacc_eff) * 128u * 128u);
             for (int s = 0; s < nacc_eff; ++s)
-              ptx::tma_load_5d(dst + s * 16384, &tmA, &fullA[slot], cb * 64, tc.w0 + s * 128, 0, ti, xb);
+              ptx::tma_load_5d(dst + s * 16384, &tmA, &fullA[slot], cb * kCB, tc.w0 + s * 128, 0, ti, xb);
           } else {
             ptx::mbar_expect_tx(&fullA[slot], p.slab_bytes);
-            ptx::tma_load_5d(dst, &tmA, &fullA[slot], cb * 64, tc.w0 * p.sw + kw + p.off_w,
+            ptx::tma_load_5d(dst, &tmA, &fullA[slot], cb * kCB, tc.w0 * p.sw + kw + p.off_w,
                              tc.h0 * p.sh + hg * p.KHs + p.off_h, ti, xb);
           }
         }
         advance(p.NA);
       });
-      // fused 1x1 shortcut: the (unshifted) window of the second input, one slab per 64-channel block
+      // fused 1x1 shortcut: the (unshifted) window of the second input, one slab per channel block
       for (int cb2 = 0; cb2 < p.cblocks2; ++cb2) {
         wait_bar(&emptyA[slot], phase ^ 1);
         if (ptx::elect_one()) {
           ptx::mbar_expect_tx(&fullA[slot], p.slab_bytes);
-          ptx::tma_load_5d(sA + static_cast<size_t>(slot) * p.slab_stride, &tmA2, &fullA[slot], cb2 * 64, tc.w0, tc.h0, tc.t, xb);
+          ptx::tma_load_5d(sA + static_cast<size_t>(slot) * p.slab_stride, &tmA2, &fullA[slot], cb2 * kCB, tc.w0, tc.h0, tc.t, xb);
         }
         advance(p.NA);
       }
@@ -193,7 +198,7 @@ __global__ void __launch_bounds__(kThreads, 1)
           wait_bar(&emptyB[slot], phase ^ 1);
           if (ptx::elect_one()) {
             ptx::mbar_expect_tx(&fullB[slot], p.b_bytes);
-            ptx::tma_load_3d(sB + static_cast<size_t>(slot) * p.b_bytes, &tmB, &fullB[slot], cb * 64, tc.n0, tap);
+            ptx::tma_load_3d(sB + static_cast<size_t>(slot) * p.b_bytes, &tmB, &fullB[slot], cb * kCB, tc.n0, tap);
           }
           advance(p.NB);
         }
@@ -202,7 +207,7 @@ __global__ void __launch_bounds__(kThreads, 1)
         wait_bar(&emptyB[slot], phase ^ 1);
         if (ptx::elect_one()) {
           ptx::mbar_expect_tx(&fullB[slot], p.b_bytes);
-          ptx::tma_load_3d(sB + static_cast<size_t>(slot) * p.b_bytes, &tmB2, &fullB[slot], cb2 * 64, tc.n0, 0);
+          ptx::tma_load_3d(sB + static_cast<size_t>(slot) * p.b_bytes, &tmB2, &fullB[slot], cb2 * kCB, tc.n0, 0);
         }
         advance(p.NB);
       }
@@ -253,7 +258,7 @@ __global__ void __launch_bounds__(kThreads, 1)
             const uint32_t a_s = a_base + static_cast<uint32_t>(s) * sub_stride;
 #pragma unroll
             for (int k = 0; k < 4; ++k)
-              if (k < ksteps)   // K = 16 per MMA; channels beyond Cin are TMA zero-fill in both operands, skip those MMAs
+              if (k < ksteps)   // K = kKmma per MMA; channels beyond Cin are TMA zero-fill in both operands, skip those MMAs
                 ptx::Wgmma<DT, BN>::run(acc[s], ptx::wgmma_desc_sw128(a_s + 32u * k), ptx::wgmma_desc_sw128(b_base + 32u * k),
                                         accumulate | static_cast<uint32_t>(k));
           }
@@ -282,16 +287,16 @@ __global__ void __launch_bounds__(kThreads, 1)
     for_each_slab(p, tc.t, [&](int kt, int ti, int hg, int kw, int cb) {
       wait_bar(&fullA[slotA], phaseA);
       if (traced && slotA == 0 && phaseA == 0 && threadIdx.x == 128) trc[2] = ptx::globaltimer_ns();
-      const int ch_left = p.Cin - cb * 64;
-      const int ksteps = ch_left >= 64 ? 4 : (ch_left + 15) >> 4;
+      const int ch_left = p.Cin - cb * kCB;
+      const int ksteps = ch_left >= kCB ? 4 : (ch_left + kKmma - 1) >> kKshift;
       const uint32_t a0 = ptx::smem_u32(sA + static_cast<size_t>(slotA) * p.slab_stride) + half_off;
       for (int khs = 0; khs < p.KHs; ++khs) mma_group(a0 + static_cast<uint32_t>(khs) * tap_stride, ksteps, khs == p.KHs - 1);
       next_slab();
     });
     for (int cb2 = 0; cb2 < p.cblocks2; ++cb2) {   // fused 1x1 shortcut: row-tap 0 of the unshifted window
       wait_bar(&fullA[slotA], phaseA);
-      const int ch_left = p.Cin2 - cb2 * 64;
-      const int ksteps = ch_left >= 64 ? 4 : (ch_left + 15) >> 4;
+      const int ch_left = p.Cin2 - cb2 * kCB;
+      const int ksteps = ch_left >= kCB ? 4 : (ch_left + kKmma - 1) >> kKshift;
       mma_group(ptx::smem_u32(sA + static_cast<size_t>(slotA) * p.slab_stride) + half_off, ksteps, true);
       next_slab();
     }
@@ -379,7 +384,7 @@ __global__ void __launch_bounds__(kThreads, 1)
         }
       }
     };
-    // Interior tiles (every row and channel valid, 16-bit output stored as channel-pair words, bias along N) take a
+    // Interior tiles (every row and channel valid, output in the activation dtype stored as channel-pair words, bias along N) take a
     // loop without per-element tests.  The general loop's branches kept ptxas from batching the bias / residual loads
     // and the stores, so its epilogue took a third of a CTA's time.  Same operations in the same order: same bits.
     const bool interior = nacc_eff == kMaxAcc && tc.n0 + BN <= p.Cout && !out_f32 && p.vec2 && !bias_m &&
@@ -405,12 +410,12 @@ __global__ void __launch_bounds__(kThreads, 1)
               float a1 = fmaf(acc[s][4 * j + 2 * rr + 1], p.alpha, b1);
               const long long off = roff[s][rr] + coff;
               if (p.residual) {
-                const float2 rf = E::to_f2(__ldg(reinterpret_cast<const unsigned int*>(reinterpret_cast<const T*>(p.residual) + off)));
+                const float2 rf = E::to_f2(__ldg(reinterpret_cast<const typename E::P*>(reinterpret_cast<const T*>(p.residual) + off)));
                 a0 += rf.x;
                 a1 += rf.y;
               }
-              const uint32_t o = E::pack2(a0, a1);
-              *reinterpret_cast<uint32_t*>(reinterpret_cast<T*>(p.y) + off) = o;
+              const typename E::P o = E::pack2(a0, a1);
+              *reinterpret_cast<typename E::P*>(reinterpret_cast<T*>(p.y) + off) = o;
               const float2 of = E::to_f2(o);
               gs0 += of.x;
               gq0 = fmaf(of.x, of.x, gq0);
@@ -464,12 +469,12 @@ __global__ void __launch_bounds__(kThreads, 1)
             const T* rp = p.residual ? reinterpret_cast<const T*>(p.residual) + off : nullptr;
             if (p.vec2 && c1ok) {
               if (rp) {
-                const float2 rf = E::to_f2(__ldg(reinterpret_cast<const unsigned int*>(rp)));
+                const float2 rf = E::to_f2(__ldg(reinterpret_cast<const typename E::P*>(rp)));
                 a0 += rf.x;
                 a1 += rf.y;
               }
-              const uint32_t o = E::pack2(a0, a1);
-              *reinterpret_cast<uint32_t*>(yp) = o;
+              const typename E::P o = E::pack2(a0, a1);
+              *reinterpret_cast<typename E::P*>(yp) = o;
               const float2 of = E::to_f2(o);
               a0 = of.x;
               a1 = of.y;
@@ -522,7 +527,7 @@ __global__ void __launch_bounds__(kThreads, 1)
 // descriptor cache keyed by (ptr, shape)").
 struct TmapKey {
   const void* ptr;
-  uint32_t rank, swizzle;
+  uint32_t rank, swizzle, esz;
   cuuint64_t dims[5], strides[4];
   cuuint32_t box[5], estr[5];
   bool operator==(const TmapKey& o) const { return memcmp(this, &o, sizeof(TmapKey)) == 0; }
@@ -534,8 +539,12 @@ struct TmapSlot {
 };
 static constexpr int kTmapSlots = 1024;
 
+// Element size of an activation dtype in bytes, and channels per 128-byte operand row.
+static int elem_bytes(int dtype) { return dtype == CVVAE_F32 ? 4 : 2; }
+static int chan_block(int dtype) { return 128 / elem_bytes(dtype); }
+
 static bool encode_map(CUtensorMap* m, const void* ptr, int rank, const cuuint64_t* dims, const cuuint64_t* strides_b,
-                       const cuuint32_t* box, const cuuint32_t* estr,
+                       const cuuint32_t* box, const cuuint32_t* estr, int esz,
                        CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
   static thread_local TmapSlot* cache = nullptr;
   if (!cache) cache = static_cast<TmapSlot*>(calloc(kTmapSlots, sizeof(TmapSlot)));
@@ -544,6 +553,7 @@ static bool encode_map(CUtensorMap* m, const void* ptr, int rank, const cuuint64
   key.ptr = ptr;
   key.rank = static_cast<uint32_t>(rank);
   key.swizzle = static_cast<uint32_t>(swizzle);
+  key.esz = static_cast<uint32_t>(esz);
   for (int i = 0; i < rank; ++i) {
     key.dims[i] = dims[i];
     key.box[i] = box[i];
@@ -563,7 +573,7 @@ static bool encode_map(CUtensorMap* m, const void* ptr, int rank, const cuuint64
     set_error("cuTensorMapEncodeTiled entry point not available");
     return false;
   }
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_UINT16, rank, const_cast<void*>(ptr), dims, strides_b, box, estr,
+  CUresult r = enc(m, esz == 4 ? CU_TENSOR_MAP_DATA_TYPE_UINT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16, rank, const_cast<void*>(ptr), dims, strides_b, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
@@ -665,7 +675,7 @@ static int conv_tc_plan(const cvvae_conv_desc* d, ConvTcParams& p, size_t& smem,
   // channel pairs as one word: unit channel stride, even position strides, word-aligned pointers
   {
     const bool out_f32 = (d->flags & CVVAE_CONV_OUT_F32) != 0;
-    const uintptr_t align = out_f32 ? 8 : 4;
+    const uintptr_t align = (out_f32 || d->dtype == CVVAE_F32) ? 8 : 4;
     p.vec2 = (y.s_c == 1) && !(y.s_w % 2) && !(y.s_h % 2) && !(y.s_t % 2) && !(y.s_b % 2) &&
              (reinterpret_cast<uintptr_t>(y.ptr) % align == 0) &&
              (!d->residual || reinterpret_cast<uintptr_t>(d->residual) % align == 0);
@@ -681,7 +691,8 @@ static int conv_tc_plan(const cvvae_conv_desc* d, ConvTcParams& p, size_t& smem,
   p.flat = (p.H_out == 1 && d->KH == 1 && d->KW == 1 && d->sw == 1 && d->sh == 1 && x.H == 1) ? 1 : 0;
   if (d->flags & (CVVAE_CONV_W_PER_BATCH | CVVAE_CONV_X_SHARED))
     CVVAE_CHECK_ARG(p.flat, "conv: batched-GEMM flags need a flat problem (H == 1, 1x1x1, stride 1)");
-  p.cblocks = (p.Cin + 63) / 64;
+  const int cb = chan_block(d->dtype);
+  p.cblocks = (p.Cin + cb - 1) / cb;
   for (;;) {
     if (p.flat) {
       p.TW = 128; p.ROWS = 1; p.TH = 1;
@@ -752,6 +763,8 @@ int conv_tc_launch(const cvvae_conv_desc* d, cudaStream_t stream) {
   const cvvae_tensor5& x = d->x;
   const cvvae_tensor5& y = d->y;
   const int N_cta = p.N_cta;
+  const int esz = elem_bytes(d->dtype);
+  const int cb = chan_block(d->dtype);
   p.trace = g_trace_buf;
   p.trace_n = g_trace_n;
 
@@ -759,12 +772,12 @@ int conv_tc_launch(const cvvae_conv_desc* d, cudaStream_t stream) {
   CUtensorMap tmA, tmB;
   {
     cuuint64_t dims[5] = {(cuuint64_t)x.C, (cuuint64_t)x.W, (cuuint64_t)x.H, (cuuint64_t)x.T, (cuuint64_t)x.B};
-    cuuint64_t strides[4] = {(cuuint64_t)x.s_w * 2, (cuuint64_t)x.s_h * 2, (cuuint64_t)x.s_t * 2, (cuuint64_t)x.s_b * 2};
+    cuuint64_t strides[4] = {(cuuint64_t)x.s_w * esz, (cuuint64_t)x.s_h * esz, (cuuint64_t)x.s_t * esz, (cuuint64_t)x.s_b * esz};
     // degenerate dims may carry meaningless strides; TMA wants multiples of 16 and monotone-ish validity
     for (int i = 0; i < 4; ++i)
-      if (dims[i + 1] == 1 && (strides[i] == 0 || strides[i] % 16)) strides[i] = (cuuint64_t)x.C * 2;
+      if (dims[i + 1] == 1 && (strides[i] == 0 || strides[i] % 16)) strides[i] = (cuuint64_t)x.C * esz;
     cuuint32_t box[5], estr[5] = {1, (cuuint32_t)d->sw, (cuuint32_t)d->sh, 1, 1};
-    box[0] = 64;
+    box[0] = (cuuint32_t)cb;
     if (p.flat) {
       box[1] = 128; box[2] = 1;
     } else {
@@ -772,15 +785,15 @@ int conv_tc_launch(const cvvae_conv_desc* d, cudaStream_t stream) {
       box[2] = (cuuint32_t)(p.slab_rows * d->sh);
     }
     box[3] = 1; box[4] = 1;
-    if (!encode_map(&tmA, x.ptr, 5, dims, strides, box, estr)) return CVVAE_E_CUDA;
+    if (!encode_map(&tmA, x.ptr, 5, dims, strides, box, estr, esz)) return CVVAE_E_CUDA;
   }
   {
     const int taps = (d->flags & CVVAE_CONV_W_PER_BATCH) ? x.B > y.B ? x.B : y.B : d->KT * d->KH * d->KW;
     cuuint64_t dims[3] = {(cuuint64_t)p.Cin, (cuuint64_t)p.Cout, (cuuint64_t)taps};
     const cuuint64_t wld = d->w_ld ? (cuuint64_t)d->w_ld : (cuuint64_t)p.Cin;
-    cuuint64_t strides[2] = {wld * 2, wld * p.Cout * 2};
-    cuuint32_t box[3] = {64, (cuuint32_t)N_cta, 1}, estr[3] = {1, 1, 1};
-    if (!encode_map(&tmB, d->w, 3, dims, strides, box, estr)) return CVVAE_E_CUDA;
+    cuuint64_t strides[2] = {wld * esz, wld * p.Cout * esz};
+    cuuint32_t box[3] = {(cuuint32_t)cb, (cuuint32_t)N_cta, 1}, estr[3] = {1, 1, 1};
+    if (!encode_map(&tmB, d->w, 3, dims, strides, box, estr, esz)) return CVVAE_E_CUDA;
   }
 
   // ---- fused 1x1 shortcut: a second input tensor (same positions as the output) and a [Cout][Cin2] matrix
@@ -800,20 +813,20 @@ int conv_tc_launch(const cvvae_conv_desc* d, cudaStream_t stream) {
     CVVAE_CHECK_ARG(-d->off_h >= 0 && -d->off_h < d->KH && -d->off_w >= 0 && -d->off_w < d->KW && d->off_t <= 0 && -d->off_t < d->KT,
                     "conv: fused shortcut needs the centre tap inside the kernel window");
     p.Cin2 = x2.C;
-    p.cblocks2 = (x2.C + 63) / 64;
+    p.cblocks2 = (x2.C + cb - 1) / cb;
     {
       cuuint64_t dims[5] = {(cuuint64_t)x2.C, (cuuint64_t)x2.W, (cuuint64_t)x2.H, (cuuint64_t)x2.T, (cuuint64_t)x2.B};
-      cuuint64_t strides[4] = {(cuuint64_t)x2.s_w * 2, (cuuint64_t)x2.s_h * 2, (cuuint64_t)x2.s_t * 2, (cuuint64_t)x2.s_b * 2};
+      cuuint64_t strides[4] = {(cuuint64_t)x2.s_w * esz, (cuuint64_t)x2.s_h * esz, (cuuint64_t)x2.s_t * esz, (cuuint64_t)x2.s_b * esz};
       for (int i = 0; i < 4; ++i)
-        if (dims[i + 1] == 1 && (strides[i] == 0 || strides[i] % 16)) strides[i] = (cuuint64_t)x2.C * 2;
-      cuuint32_t box[5] = {64, (cuuint32_t)p.TW, (cuuint32_t)p.slab_rows, 1, 1}, estr[5] = {1, 1, 1, 1, 1};
-      if (!encode_map(&tmA2, x2.ptr, 5, dims, strides, box, estr)) return CVVAE_E_CUDA;
+        if (dims[i + 1] == 1 && (strides[i] == 0 || strides[i] % 16)) strides[i] = (cuuint64_t)x2.C * esz;
+      cuuint32_t box[5] = {(cuuint32_t)cb, (cuuint32_t)p.TW, (cuuint32_t)p.slab_rows, 1, 1}, estr[5] = {1, 1, 1, 1, 1};
+      if (!encode_map(&tmA2, x2.ptr, 5, dims, strides, box, estr, esz)) return CVVAE_E_CUDA;
     }
     {
       cuuint64_t dims[3] = {(cuuint64_t)x2.C, (cuuint64_t)p.Cout, 1};
-      cuuint64_t strides[2] = {(cuuint64_t)x2.C * 2, (cuuint64_t)x2.C * p.Cout * 2};
-      cuuint32_t box[3] = {64, (cuuint32_t)N_cta, 1}, estr[3] = {1, 1, 1};
-      if (!encode_map(&tmB2, d->w2, 3, dims, strides, box, estr)) return CVVAE_E_CUDA;
+      cuuint64_t strides[2] = {(cuuint64_t)x2.C * esz, (cuuint64_t)x2.C * p.Cout * esz};
+      cuuint32_t box[3] = {(cuuint32_t)cb, (cuuint32_t)N_cta, 1}, estr[3] = {1, 1, 1};
+      if (!encode_map(&tmB2, d->w2, 3, dims, strides, box, estr, esz)) return CVVAE_E_CUDA;
     }
   }
 

@@ -1,10 +1,12 @@
 // GroupNorm(32) statistics + fused normalise/affine/SiLU, and the token LayerNorm of the temporal
-// attention.  HBM-bound kernels: 128-bit loads/stores, ~8 CTAs per SM, statistics reduced thread (fp32) -> block
+// attention.  HBM-bound kernels: 128-bit loads/stores (8 channels per thread: one vector in 16-bit storage, two in
+// fp32), ~8 CTAs per SM, statistics reduced thread (fp32) -> block
 // (shared 64-bit fixed-point atomics) -> device (global 64-bit fixed-point atomics; order-independent, reproducible).
 //
 // Replaces Normalize()+nonlinearity (reference models/vae_models.py:187-195,392-401), nn.GroupNorm+nn.SiLU
 // of models/vae_blocks3d_sd3.py, and norm_t (models/vae_models.py:571).  One rounding to 16 bit at the
-// end instead of the reference's three (GN out, sigmoid, product).
+// end instead of the reference's three (GN out, sigmoid, product).  In fp32 storage the outputs feed only convolutions, so
+// they are stored rounded to the nearest TF32 value (Elem::mma_in).
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -43,7 +45,7 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const GnView v, unsigned 
   const int unit = blockIdx.y;  // b or b*T+t
   const int b = v.per_frame ? unit / v.T : unit;
   const int ut = v.per_frame ? unit % v.T : 0;
-  const int vecs = v.C >> 3;          // 16-byte vectors per position
+  const int vecs = v.C >> 3;          // 8-channel vectors per position
   const int lanes = 256 / vecs;       // positions per sweep
   const int vec = threadIdx.x % vecs;
   const int pl = threadIdx.x / vecs;
@@ -64,39 +66,29 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const GnView v, unsigned 
     // 4 independent 128-bit loads in flight per thread (HBM latency x bandwidth needs ~35 KB in flight per SM)
     constexpr int U = 4;
     long long p = p0 + pl;
+    auto add = [&](const Vec8<DT>& u) {
+      float f[8];
+      unpack8<DT>(u, f);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        s[j] += f[j];
+        q[j] = fmaf(f[j], f[j], q[j]);
+      }
+    };
     for (; p + static_cast<long long>(U - 1) * lanes < p1; p += static_cast<long long>(U) * lanes) {
-      uint4 u[U];
+      Vec8<DT> u[U];
 #pragma unroll
       for (int i = 0; i < U; ++i) {
         const long long off = gn_offset(p + static_cast<long long>(i) * lanes, ut, v.per_frame, v.H, v.W, v.xs_t, v.xs_h,
                                         v.xs_w, v.x_dense, v.C);
-        u[i] = __ldg(reinterpret_cast<const uint4*>(xb + off + vec * 8));
+        u[i] = ld8<DT>(xb + off + vec * 8);
       }
 #pragma unroll
-      for (int i = 0; i < U; ++i) {
-        const uint32_t uw[4] = {u[i].x, u[i].y, u[i].z, u[i].w};
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float2 f = E::to_f2(uw[j]);
-          s[2 * j] += f.x;
-          q[2 * j] = fmaf(f.x, f.x, q[2 * j]);
-          s[2 * j + 1] += f.y;
-          q[2 * j + 1] = fmaf(f.y, f.y, q[2 * j + 1]);
-        }
-      }
+      for (int i = 0; i < U; ++i) add(u[i]);
     }
     for (; p < p1; p += lanes) {
       const long long off = gn_offset(p, ut, v.per_frame, v.H, v.W, v.xs_t, v.xs_h, v.xs_w, v.x_dense, v.C);
-      const uint4 u = __ldg(reinterpret_cast<const uint4*>(xb + off + vec * 8));
-      const uint32_t uw[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 f = E::to_f2(uw[j]);
-        s[2 * j] += f.x;
-        q[2 * j] = fmaf(f.x, f.x, q[2 * j]);
-        s[2 * j + 1] += f.y;
-        q[2 * j + 1] = fmaf(f.y, f.y, q[2 * j + 1]);
-      }
+      add(ld8<DT>(xb + off + vec * 8));
     }
     // fold the 8 channels of this thread into their group(s)
     if (cpg >= 8) {
@@ -138,6 +130,21 @@ __device__ __forceinline__ uint4 ld_stream(const void* p) {
 }
 __device__ __forceinline__ void st_stream(void* p, const uint4& v) {
   asm volatile("st.global.cs.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+// 8 channels, plain (__ldg / st) or streaming (no-allocate / evict-first) accesses
+template <int DT, int HINT>
+__device__ __forceinline__ Vec8<DT> ld8_hint(const typename Elem<DT>::T* p) {
+  if (!HINT) return ld8<DT>(p);
+  Vec8<DT> r;
+#pragma unroll
+  for (int i = 0; i < Vec8<DT>::kN; ++i) r.v[i] = ld_stream(reinterpret_cast<const uint4*>(p) + i);
+  return r;
+}
+template <int DT, int HINT>
+__device__ __forceinline__ void st8_hint(typename Elem<DT>::T* p, const Vec8<DT>& r) {
+  if (!HINT) return st8<DT>(p, r);
+#pragma unroll
+  for (int i = 0; i < Vec8<DT>::kN; ++i) st_stream(reinterpret_cast<uint4*>(p) + i, r.v[i]);
 }
 
 template <int DT, int U, int HINT>
@@ -182,43 +189,35 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const GnView v, const lon
   if (p1 > v.pix_per_unit) p1 = v.pix_per_unit;
   const typename E::T* xb = reinterpret_cast<const typename E::T*>(v.x) + b * v.xs_b;
   typename E::T* yb = reinterpret_cast<typename E::T*>(v.y) + b * v.ys_b;
-  auto transform = [&](const uint4& u) {
-    const uint32_t uw[4] = {u.x, u.y, u.z, u.w};
-    uint32_t ow[4];
+  auto transform = [&](const Vec8<DT>& u) {
+    float f[8];
+    unpack8<DT>(u, f);
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float2 f = E::to_f2(uw[j]);
-      float r0 = fmaf(f.x, a[2 * j], sh[2 * j]);
-      float r1 = fmaf(f.y, a[2 * j + 1], sh[2 * j + 1]);
-      if (silu) {
-        r0 = silu_f(r0);
-        r1 = silu_f(r1);
-      }
-      ow[j] = E::pack2(r0, r1);
+    for (int j = 0; j < 8; ++j) {
+      float r = fmaf(f[j], a[j], sh[j]);
+      if (silu) r = silu_f(r);
+      f[j] = E::mma_in(r);
     }
-    return make_uint4(ow[0], ow[1], ow[2], ow[3]);
+    return pack8<DT>(f);
   };
-  long long p = p0 + pl;   // U independent 128-bit loads in flight per thread
+  long long p = p0 + pl;   // U independent 8-channel loads in flight per thread
   for (; p + static_cast<long long>(U - 1) * lanes < p1; p += static_cast<long long>(U) * lanes) {
-    uint4 u[U];
+    Vec8<DT> u[U];
     long long yo[U];
 #pragma unroll
     for (int i = 0; i < U; ++i) {
       const long long pp = p + static_cast<long long>(i) * lanes;
       const long long xo = gn_offset(pp, ut, v.per_frame, v.H, v.W, v.xs_t, v.xs_h, v.xs_w, v.x_dense, v.C);
       yo[i] = gn_offset(pp, ut, v.per_frame, v.H, v.W, v.ys_t, v.ys_h, v.ys_w, v.y_dense, v.C);
-      u[i] = HINT ? ld_stream(xb + xo + vec * 8) : __ldg(reinterpret_cast<const uint4*>(xb + xo + vec * 8));
+      u[i] = ld8_hint<DT, HINT>(xb + xo + vec * 8);
     }
 #pragma unroll
-    for (int i = 0; i < U; ++i) {
-      if (HINT) st_stream(yb + yo[i] + vec * 8, transform(u[i]));
-      else *reinterpret_cast<uint4*>(yb + yo[i] + vec * 8) = transform(u[i]);
-    }
+    for (int i = 0; i < U; ++i) st8_hint<DT, HINT>(yb + yo[i] + vec * 8, transform(u[i]));
   }
   for (; p < p1; p += lanes) {
     const long long xo = gn_offset(p, ut, v.per_frame, v.H, v.W, v.xs_t, v.xs_h, v.xs_w, v.x_dense, v.C);
     const long long yo = gn_offset(p, ut, v.per_frame, v.H, v.W, v.ys_t, v.ys_h, v.ys_w, v.y_dense, v.C);
-    *reinterpret_cast<uint4*>(yb + yo + vec * 8) = transform(__ldg(reinterpret_cast<const uint4*>(xb + xo + vec * 8)));
+    st8<DT>(yb + yo + vec * 8, transform(ld8<DT>(xb + xo + vec * 8)));
   }
 }
 
@@ -288,15 +287,9 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const GnView v, long lon
   for (int i = 0; i < MAXV; ++i) {
     const int vi = lane + i * 32;
     if (vi < vecs) {
-      const uint4 u = __ldg(reinterpret_cast<const uint4*>(xp + vi * 8));
-      const uint32_t uw[4] = {u.x, u.y, u.z, u.w};
+      unpack8<DT>(ld8<DT>(xp + vi * 8), f[i]);
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 t2 = E::to_f2(uw[j]);
-        f[i][2 * j] = t2.x;
-        f[i][2 * j + 1] = t2.y;
-        sum += t2.x + t2.y;
-      }
+      for (int j = 0; j < 4; ++j) sum += f[i][2 * j] + f[i][2 * j + 1];
     }
   }
 #pragma unroll
@@ -321,15 +314,13 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const GnView v, long lon
   for (int i = 0; i < MAXV; ++i) {
     const int vi = lane + i * 32;
     if (vi < vecs) {
-      uint32_t ow[4];
+      float r[8];
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int c = vi * 8 + 2 * j;
-        const float r0 = (f[i][2 * j] - mean) * rstd * __ldg(gamma + c) + __ldg(beta + c);
-        const float r1 = (f[i][2 * j + 1] - mean) * rstd * __ldg(gamma + c + 1) + __ldg(beta + c + 1);
-        ow[j] = E::pack2(r0, r1);
+      for (int j = 0; j < 8; ++j) {
+        const int c = vi * 8 + j;
+        r[j] = E::mma_in((f[i][j] - mean) * rstd * __ldg(gamma + c) + __ldg(beta + c));
       }
-      *reinterpret_cast<uint4*>(yp + vi * 8) = make_uint4(ow[0], ow[1], ow[2], ow[3]);
+      st8<DT>(yp + vi * 8, pack8<DT>(r));
     }
   }
 }

@@ -106,7 +106,7 @@ extern "C" int cvvae_video_resize_u8(const uint8_t* thwc, uint8_t* out_thwc, voi
   const long long n = 1ll * T * OH * OW;
   const unsigned blocks = static_cast<unsigned>(n / 256 + 1 < 16ll * num_sms() ? n / 256 + 1 : 16ll * num_sms());
   const float sh = static_cast<float>(H) / static_cast<float>(OH), sw = static_cast<float>(W) / static_cast<float>(OW);
-  CVVAE_DISPATCH_DTYPE(dtype, {
+  CVVAE_DISPATCH_DTYPE16(dtype, "video_io", {
     resize_u8_kernel<DT><<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
         thwc, out_thwc, reinterpret_cast<typename Elem<DT>::T*>(out_cthw), T, H, W, OH, OW, sh, sw);
   });
@@ -119,7 +119,7 @@ extern "C" int cvvae_video_u8_to_f16(const uint8_t* thwc, void* out_cthw, int32_
   CVVAE_CHECK_ARG(thwc && out_cthw && T > 0 && H > 0 && W > 0, "cvvae_video_u8_to_f16: bad argument");
   const long long thw = 1ll * T * H * W;
   const unsigned blocks = static_cast<unsigned>(thw / 256 + 1 < 16ll * num_sms() ? thw / 256 + 1 : 16ll * num_sms());
-  CVVAE_DISPATCH_DTYPE(dtype, {
+  CVVAE_DISPATCH_DTYPE16(dtype, "video_io", {
     u8_to_f16_kernel<DT><<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
         thwc, reinterpret_cast<typename Elem<DT>::T*>(out_cthw), thw);
   });
@@ -132,7 +132,7 @@ extern "C" int cvvae_video_f16_to_u8(const void* in_cthw, uint8_t* thwc, int32_t
   CVVAE_CHECK_ARG(thwc && in_cthw && T > 0 && H > 0 && W > 0, "cvvae_video_f16_to_u8: bad argument");
   const long long thw = 1ll * T * H * W;
   const unsigned blocks = static_cast<unsigned>(thw / 256 + 1 < 16ll * num_sms() ? thw / 256 + 1 : 16ll * num_sms());
-  CVVAE_DISPATCH_DTYPE(dtype, {
+  CVVAE_DISPATCH_DTYPE16(dtype, "video_io", {
     f16_to_u8_kernel<DT><<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
         reinterpret_cast<const typename Elem<DT>::T*>(in_cthw), thwc, thw);
   });

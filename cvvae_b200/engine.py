@@ -101,11 +101,13 @@ def prepack_params(state_dict: Dict[str, torch.Tensor], ops, dtype: torch.dtype)
                 if 9 * ci_real <= 64:
                     cp = 32 if 9 * ci_real <= 32 else 64
                     w0 = state_dict[k].detach().to(dtype)
-                    wp = torch.zeros((w0.shape[2], w0.shape[0], cp), dtype=dtype, device=v.device)
-                    wp[:, :, : 9 * ci_real] = w0.permute(2, 0, 3, 4, 1).reshape(w0.shape[2], w0.shape[0], 9 * ci_real)
-                    packed[k + ".hwpack"] = wp.contiguous()
-            if k == "decoder.conv_out.weight" and v.dim() == 5 and v.shape[0] <= 4 and tuple(v.shape[3:]) == (3, 3):
-                # tap-stacked form for the tiny-Cout kernel: [KT][80][Cin], row (kh*3+kw)*8 + c
+                    wp = torch.zeros((w0.shape[0], cp, w0.shape[2]), dtype=dtype, device=v.device)
+                    wp[:, : 9 * ci_real] = w0.permute(0, 3, 4, 1, 2).reshape(w0.shape[0], 9 * ci_real, w0.shape[2])
+                    packed[k + ".hwpack"] = ops.pack_weight(wp)   # [Co, cp, KT] -> [KT, Co, cp]
+            if (k == "decoder.conv_out.weight" and v.dim() == 5 and v.shape[0] <= 4 and tuple(v.shape[3:]) == (3, 3)
+                    and dtype in (torch.float16, torch.bfloat16)):
+                # tap-stacked form for the tiny-Cout kernel: [KT][80][Cin], row (kh*3+kw)*8 + c.  That kernel is 16-bit
+                # only; an fp32 conv_out runs through the general tensor-core convolution
                 co, ci, kt = v.shape[0], v.shape[1], v.shape[2]
                 stk = torch.zeros((kt, 80, ci), dtype=dtype, device=v.device)
                 stk[:, :72].view(kt, 9, 8, ci)[:, :, :co] = v.permute(2, 3, 4, 0, 1).reshape(kt, 9, co, ci)
@@ -129,7 +131,7 @@ class Engine:
         self.hw_mode = PAD_REPLICATE if self.sd3 else PAD_ZERO
         self._stats_arena = None   # [slots, B, groups, 2] int64, zeroed once per network pass
         self._stats_next = 0
-        self.attn_scratch_bytes = 4 << 30  # cap of the fp32 logits buffer of the batched spatial attention
+        self.attn_scratch_bytes = 4 << 30  # cap of the fp32 logits buffer (with fp32 P: logits + P) of the batched spatial attention
         # 1x1 shortcuts as extra K steps of conv2 (CVVAE_FUSE_SHORTCUT=0: separate launch + residual add, for A/B runs)
         self.fuse_shortcut = os.environ.get("CVVAE_FUSE_SHORTCUT", "1") != "0"
 
@@ -294,7 +296,8 @@ class Engine:
         if key not in self.p:
             w4 = w.view(kt, khw, w.shape[1], w.shape[2])
             if pad_t == PAD_REPLICATE:
-                wf = w4.float().sum(0).to(w.dtype)      # one rounding of the fp32 sum
+                # one rounding of the fp32 sum, stored like every packed weight ([Co, Ci, khw] -> [khw, Co, Ci])
+                wf = self.ops.pack_weight(w4.float().sum(0).to(w.dtype).permute(1, 2, 0))
             elif 0 <= tl < kt:
                 wf = w4[tl]
             else:
@@ -372,7 +375,7 @@ class Engine:
         one right operand per frame) and one row softmax over all frames:
           v^T = W_v hn^T + b_v   (left operand W_v shared by the frames, bias along rows; gives the K-major operand of
                                   the last GEMM directly)
-          S   = q k^T * C^-0.5   (fp32 logits) ; P = softmax(S) (16 bit)
+          S   = q k^T * C^-0.5   (fp32 logits) ; P = softmax(S) (activation dtype)
           O   = P v
         Frames are processed in groups so that the fp32 logits stay below `attn_scratch_bytes`.
         """
@@ -384,7 +387,9 @@ class Engine:
         out = ops.empty((B, T, H, W, Cc), hn.dtype, hn.device)
         wv_act = wv.view(1, 1, 1, Cc, Cc)
         scale = float(Cc) ** -0.5
-        fg = max(1, min(F, self.attn_scratch_bytes // max(1, N * ld * 4)))
+        # S is fp32; a 16-bit P is half its size and not counted, an fp32 P doubles the scratch and is
+        per_frame = N * ld * (4 + hn.element_size() if hn.element_size() == 4 else 4)
+        fg = max(1, min(F, self.attn_scratch_bytes // max(1, per_frame)))
         vT = ops.empty((fg, Cc, ld), hn.dtype, hn.device)
         S = torch.empty((fg, N, ld), dtype=torch.float32, device=hn.device)
         P = ops.empty((fg, N, ld), hn.dtype, hn.device)

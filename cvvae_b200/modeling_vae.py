@@ -231,8 +231,8 @@ class _CVVAEBase(nn.Module):
                 if p0.device.type != "cuda":
                     raise RuntimeError("cvvae_b200 runs on CUDA (sm_90a) only: move the model with .cuda(); "
                                        "there is no CPU or PyTorch fallback path")
-                if p0.dtype not in (torch.float16, torch.bfloat16):
-                    raise RuntimeError(f"cvvae_b200 computes in float16/bfloat16; model dtype is {p0.dtype} - call .half()")
+                if p0.dtype not in (torch.float16, torch.bfloat16, torch.float32):
+                    raise RuntimeError(f"cvvae_b200 computes in float16, bfloat16 or float32; model dtype is {p0.dtype}")
                 from .ops import CudaOps
                 ops = CudaOps()
             packed = prepack_params(self.state_dict(), ops, p0.dtype)

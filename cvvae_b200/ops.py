@@ -17,14 +17,14 @@ import torch
 
 from . import _lib as L
 
-_DT = {torch.float16: L.F16, torch.bfloat16: L.BF16}
+_DT = {torch.float16: L.F16, torch.bfloat16: L.BF16, torch.float32: L.F32}
 
 
 def dtype_code(dt: torch.dtype) -> int:
     try:
         return _DT[dt]
     except KeyError:
-        raise L.CvvaeError(f"cvvae_b200 computes in float16 or bfloat16 only, got {dt}; call .half() or .bfloat16()")
+        raise L.CvvaeError(f"cvvae_b200 computes in float16, bfloat16 or float32 (TF32 tensor-core products), got {dt}")
 
 
 def _t5(t: torch.Tensor) -> L.Tensor5:
@@ -103,7 +103,7 @@ class CudaOps:
     # ------------------------------------------------------------------ convolution / GEMM
     @_on_tensor_device
     def pack_weight(self, w: torch.Tensor) -> torch.Tensor:
-        """[Cout, Cin, *k] (PyTorch) -> [taps, Cout, Cin] in the same 16-bit dtype."""
+        """[Cout, Cin, *k] (PyTorch) -> [taps, Cout, Cin] in the same dtype (fp32: rounded to the nearest TF32 value)."""
         w = w.contiguous()
         co, ci = w.shape[0], w.shape[1]
         taps = 1
@@ -294,7 +294,7 @@ class CudaOps:
     # ------------------------------------------------------------------ attention helpers
     @_on_tensor_device
     def softmax_rows(self, s: torch.Tensor, cols: int, out: torch.Tensor) -> torch.Tensor:
-        """s: fp32 [rows, ld_s]; out: 16-bit [rows, ld_p]; softmax over the first `cols` of each row."""
+        """s: fp32 [rows, ld_s]; out: activation dtype [rows, ld_p]; softmax over the first `cols` of each row."""
         assert s.dtype == torch.float32 and s.dim() == 2 and out.dim() == 2 and s.stride(1) == 1 and out.stride(1) == 1
         L.check(self.lib.cvvae_softmax_rows(s.data_ptr(), s.stride(0), out.data_ptr(), out.stride(0), s.shape[0], cols,
                                             dtype_code(out.dtype), _stream(s)), "cvvae_softmax_rows")

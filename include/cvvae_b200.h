@@ -14,8 +14,14 @@
  *   - every call is asynchronous on the `stream` it is given (a cudaStream_t passed as void*).
  *   - activations are channels-last: element (b,t,h,w,c) lives at b*s_b + t*s_t + h*s_h + w*s_w + c*s_c
  *     (strides in ELEMENTS).  The tensor-core path needs s_c == 1 on its input.
- *   - dtype: CVVAE_F16 or CVVAE_BF16 for activations and packed weights; bias / norm parameters are fp32;
+ *   - dtype: CVVAE_F16, CVVAE_BF16 or CVVAE_F32 for activations and packed weights; bias / norm parameters are fp32;
  *     GroupNorm statistics are 64-bit fixed point (order-independent integer accumulation, see below).
+ *     CVVAE_F32: activations and packed weights are fp32 and the tensor-core path multiplies in TF32 (10-bit mantissa
+ *     products, fp32 accumulation), as PyTorch's default fp32 convolution does on this GPU.  Outputs whose only
+ *     consumers are tensor-core products (packed weights, GroupNorm / LayerNorm / softmax outputs, pack_taps_hw and the
+ *     channels-first -> channels-last copy of a network input) are stored rounded to the nearest TF32 value; every other output
+ *     (convolution outputs: residual stream, q / k / v, attention output) is full fp32.  The video_io entry points and
+ *     cvvae_conv3d_stacked are 16-bit only and reject CVVAE_F32.
  */
 #ifndef CVVAE_B200_H_
 #define CVVAE_B200_H_
@@ -26,9 +32,9 @@
 extern "C" {
 #endif
 
-#define CVVAE_ABI_VERSION 2
+#define CVVAE_ABI_VERSION 3
 
-enum { CVVAE_F16 = 0, CVVAE_BF16 = 1 };
+enum { CVVAE_F16 = 0, CVVAE_BF16 = 1, CVVAE_F32 = 2 };
 enum { CVVAE_PAD_ZERO = 0, CVVAE_PAD_REPLICATE = 1 };
 enum {
   CVVAE_OK = 0,
@@ -86,10 +92,10 @@ typedef struct cvvae_conv_desc {
   int32_t off_t, off_h, off_w;
   int32_t pad_t, pad_hw;    /* CVVAE_PAD_* */
   int32_t up_time;          /* 1 or 2 */
-  int32_t dtype;            /* CVVAE_F16 / CVVAE_BF16 */
+  int32_t dtype;            /* CVVAE_F16 / CVVAE_BF16 / CVVAE_F32 */
   int32_t flags;            /* CVVAE_CONV_* */
   float alpha;
-  int64_t* gn_stats;        /* optional [B][gn_groups][2] int64 fixed point as above (of the STORED 16-bit y), accumulated:
+  int64_t* gn_stats;        /* optional [B][gn_groups][2] int64 fixed point as above (of the STORED y), accumulated:
                                GroupNorm statistics of the consumer, produced in the conv epilogue instead of a
                                separate pass over y.  The caller zeroes it (several launches may add to it).  */
   int32_t gn_groups;
@@ -117,7 +123,8 @@ int cvvae_conv3d_is_tc(const cvvae_conv_desc* d);
  * no residual / statistics / fp32 output.  pad_hw == REPLICATE needs a framed input (off_h = off_w = 0). */
 int cvvae_conv3d_stacked(const cvvae_conv_desc* d, void* stream);
 
-/* [Cout][Cin][KT][KH][KW] (PyTorch layout, contiguous, activation dtype) -> [KT*KH*KW][Cout][Cin]. */
+/* [Cout][Cin][KT][KH][KW] (PyTorch layout, contiguous, activation dtype) -> [KT*KH*KW][Cout][Cin].  CVVAE_F32: the packed
+ * weights are rounded to the nearest TF32 value. */
 int cvvae_pack_conv_weight(const void* w_oikkk, void* w_packed, int32_t Cout, int32_t Cin, int32_t taps,
                            int32_t dtype, void* stream);
 
@@ -140,7 +147,7 @@ int cvvae_groupnorm_apply(const cvvae_tensor5* x, const cvvae_tensor5* y, int32_
 int cvvae_layernorm(const cvvae_tensor5* x, const cvvae_tensor5* y, const float* gamma, const float* beta,
                     float eps, int32_t dtype, void* stream);
 
-/* Row softmax: fp32 logits s[rows][ld_s] -> 16-bit probabilities p[rows][ld_p] (first `cols` entries of
+/* Row softmax: fp32 logits s[rows][ld_s] -> probabilities p[rows][ld_p] in the activation dtype (first `cols` entries of
  * each row), fp32 math.  Part of softmax(q k^T / sqrt(C)) v (models/vae_models.py:456,518,607). */
 int cvvae_softmax_rows(const float* s, int64_t ld_s, void* p, int64_t ld_p, int64_t rows, int32_t cols,
                        int32_t dtype, void* stream);
@@ -155,7 +162,9 @@ int cvvae_attn_temporal(const cvvae_tensor5* q, const cvvae_tensor5* k, const cv
 int cvvae_replicate_border(const cvvae_tensor5* xpad, int32_t dtype, void* stream);
 
 /* Generic strided copy / layout change between two 5-D views of equal logical shape; y may have more
- * channels than x, the extra channels are zero-filled (channel padding of the 3/4-channel network inputs). */
+ * channels than x, the extra channels are zero-filled (channel padding of the 3/4-channel network inputs).
+ * CVVAE_F32: a copy from a channels-first view (x.s_c != 1) into a channels-last one (y.s_c == 1) is the gather of a
+ * network input for its first convolution and stores values rounded to the nearest TF32; every other copy is exact. */
 int cvvae_copy5(const cvvae_tensor5* x, const cvvae_tensor5* y, int32_t dtype, void* stream);
 
 /* Spatial taps of a network-input convolution packed into channels (conv_in of Encoder / Decoder: 3 / 4 input channels,
@@ -207,7 +216,7 @@ int64_t cvvae_launch_count(void);
  * 256}) whose A operand starts `row_shift` 128-byte rows into a TMA-written SWIZZLE_128B slab of 320 rows, with the given
  * base_offset field and with consecutive 8-row groups `sbo_rows` (8..16) slab rows apart.  a_rows: [320][64], out: fp32
  * [128][N].
- * (Decides how shifted conv taps may address one staged slab.) */
+ * (Decides how shifted conv taps may address one staged slab.)  16-bit dtypes only. */
 int cvvae_probe_umma_shift(const void* a_rows, const void* b_rows, float* out, int32_t n, int32_t row_shift,
                            int32_t base_offset_mode, int32_t sbo_rows, void* stream);
 

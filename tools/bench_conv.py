@@ -1,10 +1,11 @@
 #!/usr/bin/env python
 """Per-layer microbenchmark of the tensor-core convolution on the distinct conv problems of one
 17x576x576 tile (SURVEY.md section 3.6).  Prints one JSON line per problem: ms, TFLOP/s, fraction of the peak bench.py
-uses (MEASURED_PEAKS.json when present, else the H100 SXM data-sheet 989 TFLOP/s).  L2 is flushed between timed
+uses (MEASURED_PEAKS.json when present, else the H100 SXM data-sheet 989 TFLOP/s); with --dtype fp32 (TF32 products) the
+H100 SXM data-sheet dense TF32 figure, 495 TFLOP/s, labelled as such.  L2 is flushed between timed
 launches (256 MB memset) and each timing is the median of `reps`.
 
-    python tools/bench_conv.py [--reps 5] [--only substring] [--scale 1.0]
+    python tools/bench_conv.py [--reps 5] [--only substring] [--dtype fp16|bf16|fp32]
 """
 import argparse
 import json
@@ -44,15 +45,23 @@ P = [
 ]
 
 
+DTYPES = {"fp16": torch.float16, "bf16": torch.bfloat16, "fp32": torch.float32}
+TF32_PEAK_DATASHEET = 495.0   # TFLOP/s: H100 SXM data sheet, dense TF32 tensor-core rate
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--only", default="")
+    ap.add_argument("--dtype", choices=sorted(DTYPES), default="fp16")
     args = ap.parse_args()
-    peak, _ = bench.peaks()
+    dt = DTYPES[args.dtype]
+    if dt == torch.float32:
+        peak, peak_src = TF32_PEAK_DATASHEET, "H100 SXM data sheet, dense TF32"
+    else:
+        peak, peak_src = bench.peaks()[0], "bench.peaks()"
     ops = CudaOps()
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
-    dt = torch.float16
     for name, ci, co, k, s, (T, H, W), pads, pad_t, up in P:
         if args.only and args.only not in name:
             continue
@@ -86,7 +95,7 @@ def main():
         flops = 2.0 * To * Ho * Wo * co * k[0] * k[1] * k[2] * ci
         tf = flops / (ms * 1e-3) / 1e12
         print(json.dumps({"layer": name, "ms": round(ms, 3), "tflops": round(tf, 1), "frac_of_peak": round(tf / peak, 3),
-                          "gflop": round(flops / 1e9, 1)}), flush=True)
+                          "gflop": round(flops / 1e9, 1), "dtype": args.dtype, "peak_source": peak_src}), flush=True)
         del x, w, y
 
 

@@ -72,6 +72,8 @@ EXPORTS = tuple(_SIGNATURES)
 # the values cvvae_conv_tc_plan() writes, in order
 CONV_TC_PLAN_FIELDS = ("eligible", "N_cta", "NACC", "TW", "ROWS", "TH", "tiles_w", "tiles_h", "n_tiles_n", "flat", "NA", "NB",
                        "grid", "vec2")
+# ... followed by which epilogue the launch runs (1: shared-memory staging and TMA stores)
+CONV_TC_PLAN_EPILOGUE_FIELDS = CONV_TC_PLAN_FIELDS + ("tma_epilogue",)
 
 _lib = None
 

@@ -17,12 +17,15 @@
 //
 // Warpgroups (384 threads): 0 = producers (warp 0 slabs, warp 1 weights; registers handed to the MMA warpgroups),
 // 1 and 2 = MMA issue + epilogue (registers -> bias/alpha/residual -> stores in the activation dtype, with the time-interleave scatter of
-// Upsample3D folded into the store address, and the consumer GroupNorm's statistics).
+// Upsample3D folded into the store address, and the consumer GroupNorm's statistics).  16-bit channels-last outputs are
+// staged in the freed A ring and written by TMA stores; their residual is prefetched by TMA after the last slab.
 //
 // Replaces cuDNN behind CausalConv3d / nn.Conv3d / Conv2dWithExtraDim / Downsample3D / Upsample3D
 // (reference: models/vae_models.py:198-340, models/vae_blocks3d_sd3.py:16-364); see include/cvvae_b200.h.
 #include <stdlib.h>
 #include <string.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 #include "ptx.cuh"
@@ -50,6 +53,8 @@ struct ConvTcParams {
   // fused 1x1 shortcut (ResnetBlock3D nin_shortcut / conv_shortcut as extra K steps of conv2): cblocks2 channel blocks
   // of a second input tensor (same positions as the output) times a [Cout][Cin2] matrix, accumulated after the taps
   int Cin2, cblocks2;
+  // epilogue through shared memory and TMA stores (16-bit channels-last outputs), residual prefetched into the A ring
+  int tma_epi;
   unsigned long long* trace;  // optional [trace_n][8] globaltimer stamps per CTA (diagnostics)
   int trace_n;
 };
@@ -94,10 +99,37 @@ __device__ __forceinline__ void for_each_slab(const ConvTcParams& p, int t, F&& 
   }
 }
 
+// TMA epilogue: channel block c (cb channels) of the tile.  Its first channel and frame in y, or false when it has nothing
+// to write (past Cout, or the first half of the up_time = 2 interleave at t = 0).  A block never straddles the interleave
+// halves (the plan asks for Cout / 2 to be a multiple of cb).
+__device__ __forceinline__ bool epi_block(const ConvTcParams& p, const TileCoord& tc, int c, int cb, int& c0, int& t_o) {
+  const int g = tc.n0 + c * cb;
+  if (g >= p.Cout) return false;
+  const int n_il = p.up_time == 2 ? g / (p.Cout / 2) : 0;
+  c0 = g - n_il * (p.Cout / 2);
+  t_o = p.up_time == 2 ? 2 * tc.t + n_il - 1 : tc.t;
+  return t_o >= 0;
+}
+// TMA epilogue: the 64 positions s * 128 + 64 * hf of the tile (half hf of sub-tile s) are one box of the y / residual
+// maps, {cb, TW, ROWS / 2} or {cb, 64, 1}; its (w, h) corner.
+__device__ __forceinline__ void epi_piece(const ConvTcParams& p, const TileCoord& tc, int s, int hf, int& w, int& h) {
+  if (p.flat) {
+    w = tc.w0 + s * 128 + 64 * hf;
+    h = 0;
+  } else if (p.ROWS == 1) {
+    w = tc.w0 + 64 * hf;
+    h = tc.h0 + s;
+  } else {
+    w = tc.w0;
+    h = tc.h0 + s * p.ROWS + hf * (p.ROWS / 2);
+  }
+}
+
 template <int DT, int BN>
 __global__ void __launch_bounds__(kThreads, 1)
     conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                    const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
+                   const __grid_constant__ CUtensorMap tmY, const __grid_constant__ CUtensorMap tmR,
                    const ConvTcParams p) {
   constexpr int kMaxAcc = 256 / BN;   // 128-position sub-tiles per CTA at most
   constexpr int kR = BN / 2;          // accumulator registers per thread per sub-tile
@@ -144,6 +176,10 @@ __global__ void __launch_bounds__(kThreads, 1)
     ptx::fence_mbar_init();
     ptx::prefetch_tmap(&tmA);
     ptx::prefetch_tmap(&tmB);
+    if (p.tma_epi) {
+      ptx::prefetch_tmap(&tmY);
+      if (p.residual) ptx::prefetch_tmap(&tmR);
+    }
   }
   __syncthreads();
   if (traced && threadIdx.x == 0) trc[1] = ptx::globaltimer_ns();
@@ -189,6 +225,33 @@ __global__ void __launch_bounds__(kThreads, 1)
         }
         advance(p.NA);
       }
+      // TMA epilogue: claim the slots the epilogue stages the output in, one channel block per slot, and load the
+      // block's residual into it.  A slot is released as soon as both MMA warpgroups have finished reading its slab,
+      // which for all but the last slab happens while later slabs are multiplied: the residual arrives under the MMAs,
+      // and a block's staging never waits for the other warpgroup's last MMAs unless it reuses the last slab's slot.
+      if (kCB == 64 && p.tma_epi) {
+        for (int c = 0; c < BN / kCB; ++c) {
+          int c0, t_o;
+          if (epi_block(p, tc, c, kCB, c0, t_o)) {
+            wait_bar(&emptyA[slot], phase ^ 1);
+            if (ptx::elect_one()) {
+              uint8_t* dst = sA + static_cast<size_t>(slot) * p.slab_stride;
+              if (p.residual) {
+                ptx::mbar_expect_tx(&fullA[slot], static_cast<uint32_t>(nacc_eff) * 16384u);
+                for (int s = 0; s < nacc_eff; ++s)
+                  for (int hf = 0; hf < 2; ++hf) {
+                    int w, h;
+                    epi_piece(p, tc, s, hf, w, h);
+                    ptx::tma_load_5d(dst + s * 16384 + hf * 8192, &tmR, &fullA[slot], c0, w, h, t_o, tc.b);
+                  }
+              } else {
+                ptx::mbar_arrive(&fullA[slot]);
+              }
+            }
+          }
+          advance(p.NA);
+        }
+      }
     } else if (warp == 1) {
       // ------------------------------------------------------------- B producer
       for_each_slab(p, tc.t, [&](int kt, int ti, int hg, int kw, int cb) {
@@ -220,6 +283,8 @@ __global__ void __launch_bounds__(kThreads, 1)
   const int half = (threadIdx.x >> 7) - 1;           // which 64-row half of every sub-tile
   const bool wg_leader = (threadIdx.x & 127) == 0;
   float acc[kMaxAcc][kR];   // written first by an MMA with scale_d = 0; sub-tiles past nacc_eff are never read
+  int epi_slot;             // the A-ring slot after the last slab, and its phase: where the TMA epilogue's blocks start
+  uint32_t epi_phase;
   {
     int slotA = 0, slotB = 0;
     uint32_t phaseA = 0, phaseB = 0;
@@ -308,6 +373,8 @@ __global__ void __launch_bounds__(kThreads, 1)
       if (pendB >= 0) ptx::mbar_arrive(&emptyB[pendB]);
       if (pendA >= 0) ptx::mbar_arrive(&emptyA[pendA]);
     }
+    epi_slot = slotA;
+    epi_phase = phaseA;
   }
   if (traced && threadIdx.x == 128) trc[5] = ptx::globaltimer_ns();
 
@@ -387,10 +454,110 @@ __global__ void __launch_bounds__(kThreads, 1)
     // Interior tiles (every row and channel valid, output in the activation dtype stored as channel-pair words, bias along N) take a
     // loop without per-element tests.  The general loop's branches kept ptxas from batching the bias / residual loads
     // and the stores, so its epilogue took a third of a CTA's time.  Same operations in the same order: same bits.
+    const bool tma_epi = kCB == 64 && p.tma_epi;
     const bool interior = nacc_eff == kMaxAcc && tc.n0 + BN <= p.Cout && !out_f32 && p.vec2 && !bias_m &&
                           (p.flat ? tc.w0 + kMaxAcc * 128 <= p.W_out
                                   : tc.h0 + kMaxAcc * p.ROWS <= p.H_out && tc.w0 + p.TW <= p.W_out);
-    if (interior) {
+    if (tma_epi) {
+      if constexpr (kCB == 64) {
+        // Every tile, interior or edge.  Channel block c of the tile (64 channels x NACC * 128 positions, 128-B rows in
+        // SWIZZLE_128B order, i.e. the layout of the y map's boxes) is staged in A-ring slot epi_slot + c, which the A
+        // producer hands over through fullA once both warpgroups have released it, with the block's residual loaded
+        // when there is one; each thread reads its residual words and writes the result over them.  Then the
+        // warpgroup's rows go out as TMA stores, which clip whatever lies outside y: edge rows, channels past Cout.
+        // Same operations in the same order as the loops below: same bits.
+        constexpr int kBlocks = BN / kCB;
+        const int sw = lane >> 2;   // position & 7 of this thread's rows: the 16-byte chunk swizzle
+        const uint32_t row_off = static_cast<uint32_t>(half * 64 + wl * 16 + sw) * 128u + 4u * (lane & 3);
+        // The bias is loaded once, all loads in flight together: lane l holds channels n0 + 64c + 8(l/4) + 2(l%4) (+1),
+        // and the thread's channel pair j = 8c + jj comes from lane 4jj + l%4.  A load per j, issued after the previous
+        // j's work, left the loop waiting on L2 once per j.
+        float bl[kBlocks][2];
+#pragma unroll
+        for (int c = 0; c < kBlocks; ++c) {
+          const int ch = tc.n0 + c * kCB + 8 * sw + cpair;
+          bl[c][0] = p.bias && ch < p.Cout ? __ldg(p.bias + ch) : 0.f;
+          bl[c][1] = p.bias && ch + 1 < p.Cout ? __ldg(p.bias + ch + 1) : 0.f;
+        }
+        // Residual, statistics and a full set of sub-tiles are template switches of the staging loop, so that each
+        // instance is straight-line code: with runtime tests inside, every pair carried predicate juggling and the
+        // statistics arithmetic, and the loop issued several times the instructions it needs.
+        auto stage_blocks = [&](auto res_c, auto gn_c, auto full_c) {
+          constexpr bool kRes = decltype(res_c)::value, kGn = decltype(gn_c)::value, kFull = decltype(full_c)::value;
+#pragma unroll
+          for (int c = 0; c < kBlocks; ++c) {
+            int c0, t_o;
+            if (!epi_block(p, tc, c, kCB, c0, t_o)) continue;   // warp-uniform
+            const int slot = epi_slot + c < p.NA ? epi_slot + c : epi_slot + c - p.NA;
+            const uint32_t stage = ptx::smem_u32(sA + static_cast<size_t>(slot) * p.slab_stride) + row_off;
+            wait_bar(&fullA[slot], epi_slot + c < p.NA ? epi_phase : epi_phase ^ 1);
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const int j = 8 * c + jj;
+              const float b0 = __shfl_sync(0xffffffffu, bl[c][0], 4 * jj + (lane & 3));
+              const float b1 = __shfl_sync(0xffffffffu, bl[c][1], 4 * jj + (lane & 3));
+              const uint32_t chunk = stage + static_cast<uint32_t>((jj ^ sw) << 4);
+              float gs0 = 0.f, gq0 = 0.f, gs1 = 0.f, gq1 = 0.f;
+#pragma unroll
+              for (int s = 0; s < kMaxAcc; ++s) {
+                // sub-tiles past nacc_eff hold no output (and past NACC have no slot space)
+                const bool sok = kFull || s < nacc_eff;
+#pragma unroll
+                for (int rr = 0; rr < 2; ++rr) {
+                  const uint32_t addr = chunk + static_cast<uint32_t>(s * 16384 + rr * 1024);
+                  float a0 = fmaf(acc[s][4 * j + 2 * rr], p.alpha, b0);
+                  float a1 = fmaf(acc[s][4 * j + 2 * rr + 1], p.alpha, b1);
+                  if (kRes && sok) {
+                    const float2 rf = E::to_f2(ptx::ld_shared_b32(addr));
+                    a0 += rf.x;
+                    a1 += rf.y;
+                  }
+                  const uint32_t o = E::pack2(a0, a1);
+                  if (sok) ptx::st_shared_b32(addr, o);
+                  if (kGn && rok[s][rr]) {
+                    const float2 of = E::to_f2(o);
+                    gs0 += of.x;
+                    gq0 = fmaf(of.x, of.x, gq0);
+                    gs1 += of.y;
+                    gq1 = fmaf(of.y, of.y, gq1);
+                  }
+                }
+              }
+              // channels past Cout (a block that Cout ends inside; Cout % 8 == 0, so per pair) are computed from zero
+              // weights and bias, clipped by the store and kept out of the statistics
+              if (kGn) gn_add(gs0, gq0, gs1, gq1, c0 + 8 * jj + cpair, tc.n0 + 8 * j < p.Cout, true);
+            }
+          }
+        };
+        auto by_full = [&](auto res_c, auto gn_c) {
+          if (nacc_eff == kMaxAcc) stage_blocks(res_c, gn_c, std::true_type{});
+          else stage_blocks(res_c, gn_c, std::false_type{});
+        };
+        auto by_gn = [&](auto res_c) {
+          if (p.gn_stats) by_full(res_c, std::true_type{});
+          else by_full(res_c, std::false_type{});
+        };
+        if (p.residual) by_gn(std::true_type{});
+        else by_gn(std::false_type{});
+        ptx::fence_proxy_async();             // the staged words are visible to the TMA unit
+        if (half == 0) ptx::named_bar_sync(3, 128);   // this warpgroup's rows are all written
+        else ptx::named_bar_sync(4, 128);
+        if (wg_leader) {
+          for (int c = 0; c < kBlocks; ++c) {
+            int bc0, bt;
+            if (!epi_block(p, tc, c, kCB, bc0, bt)) continue;
+            const int slot = epi_slot + c < p.NA ? epi_slot + c : epi_slot + c - p.NA;
+            const uint8_t* src = sA + static_cast<size_t>(slot) * p.slab_stride + half * 8192;
+            for (int s = 0; s < nacc_eff; ++s) {
+              int w, h;
+              epi_piece(p, tc, s, half, w, h);
+              ptx::tma_store_5d(&tmY, src + s * 16384, bc0, w, h, bt, tc.b);
+            }
+          }
+          ptx::bulk_commit();
+        }
+      }
+    } else if (interior) {
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j) {
         const int cg = tc.n0 + 8 * j + cpair;
@@ -513,6 +680,8 @@ __global__ void __launch_bounds__(kThreads, 1)
         atomicAdd(reinterpret_cast<unsigned long long*>(p.gn_stats) + static_cast<size_t>(tc.b) * 2 * p.gn_groups + ct, vsum);
     }
   }
+  // the staged tile must stay in shared memory until the TMA unit has read it (not until the global writes land)
+  if (kCB == 64 && p.tma_epi && wg_leader) ptx::bulk_wait_read<0>();
   if (traced && threadIdx.x == 128) {
     unsigned smid;
     asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
@@ -624,14 +793,47 @@ void conv_tc_set_trace(unsigned long long* buf, int n) {
 
 template <int DT, int BN>
 static int launch_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmA2, const CUtensorMap& tmB2,
-                     const ConvTcParams& p, unsigned grid, size_t smem, cudaStream_t stream) {
+                     const CUtensorMap& tmY, const CUtensorMap& tmR, const ConvTcParams& p, unsigned grid, size_t smem,
+                     cudaStream_t stream) {
   static PerDeviceOnce attr_set;   // the > 48 KB shared-memory opt-in is per device
   if (attr_set.need()) {
     CVVAE_CUDA(cudaFuncSetAttribute(conv_tc_kernel<DT, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
     attr_set.mark();
   }
-  conv_tc_kernel<DT, BN><<<grid, kThreads, smem, stream>>>(tmA, tmB, tmA2, tmB2, p);
+  conv_tc_kernel<DT, BN><<<grid, kThreads, smem, stream>>>(tmA, tmB, tmA2, tmB2, tmY, tmR, p);
   return CVVAE_OK;
+}
+
+// Byte strides of y's W, H, T and B axes for a tensor map, or false when TMA cannot address y: channel stride != 1, or a
+// pointer or stride that is not a multiple of 16 bytes.  An axis of extent 1 may carry any stride; it gets a valid one.
+static bool y_map_strides(const cvvae_tensor5& y, int esz, cuuint64_t* strides) {
+  const long long s[4] = {y.s_w, y.s_h, y.s_t, y.s_b};
+  const int n[4] = {y.W, y.H, y.T, y.B};
+  if (y.s_c != 1 || reinterpret_cast<uintptr_t>(y.ptr) % 16) return false;
+  for (int i = 0; i < 4; ++i) {
+    if (n[i] == 1) {
+      strides[i] = (static_cast<cuuint64_t>(y.C) * esz + 15) & ~cuuint64_t(15);
+    } else {
+      if (s[i] <= 0 || (s[i] * esz) % 16) return false;
+      strides[i] = static_cast<cuuint64_t>(s[i]) * esz;
+    }
+  }
+  return true;
+}
+
+// The output goes through shared memory and TMA stores (and the residual comes in by TMA) when y is a 16-bit channels-last
+// tensor TMA can address, with the residual on the same strides and a block of 64 channels staged per A-ring slot (the
+// BN / 64 blocks need that many slots; a slot always holds one, since slab_rows >= TH).  fp32 outputs (logits, fp32
+// models), bias along M and the NCDHW / unaligned views keep the register epilogue, as does CVVAE_TMA_EPILOGUE=0.
+static bool tma_epilogue_ok(const cvvae_conv_desc* d, const ConvTcParams& p) {
+  const char* env = getenv("CVVAE_TMA_EPILOGUE");
+  if (env && strcmp(env, "0") == 0) return false;
+  if (d->dtype == CVVAE_F32 || (d->flags & (CVVAE_CONV_OUT_F32 | CVVAE_CONV_BIAS_ALONG_M))) return false;
+  cuuint64_t strides[4];
+  if (!y_map_strides(d->y, 2, strides)) return false;
+  if (d->residual && reinterpret_cast<uintptr_t>(d->residual) % 16) return false;
+  if (p.Cout % 8 || (p.up_time == 2 && (p.Cout / 2) % 64)) return false;
+  return p.N_cta / 64 <= p.NA;
 }
 
 // The launch plan of a descriptor: geometry, epilogue pointers and strides, tiling (N_cta, NACC, TW / TH, tile counts),
@@ -748,6 +950,7 @@ static int conv_tc_plan(const cvvae_conv_desc* d, ConvTcParams& p, size_t& smem,
   p.NA = NA;
   p.NB = NB;
   smem = 1024 + static_cast<size_t>(NA) * p.slab_stride + static_cast<size_t>(NB) * p.b_bytes + kBarBytes;
+  p.tma_epi = tma_epilogue_ok(d, p) ? 1 : 0;
 
   grid = 1ll * p.n_tiles_n * p.T_out * p.tiles_w * p.tiles_h * p.B;
   CVVAE_CHECK_ARG(grid > 0 && grid < (1ll << 31), "conv_tc: grid size %lld out of range", grid);
@@ -845,11 +1048,24 @@ int conv_tc_launch(const cvvae_conv_desc* d, cudaStream_t stream) {
     p.gn_cpg = cpg;
   }
 
+  // ---- TMA epilogue: y and the residual (same strides) as 5-D maps, one box = 64 positions x 64 channels
+  CUtensorMap tmY = tmA, tmR = tmA;
+  if (p.tma_epi) {
+    cuuint64_t dims[5] = {(cuuint64_t)y.C, (cuuint64_t)y.W, (cuuint64_t)y.H, (cuuint64_t)y.T, (cuuint64_t)y.B};
+    cuuint64_t strides[4];
+    y_map_strides(y, esz, strides);
+    const bool rows = p.ROWS >= 2;
+    cuuint32_t box[5] = {(cuuint32_t)cb, (cuuint32_t)(rows ? p.TW : 64), (cuuint32_t)(rows ? p.ROWS / 2 : 1), 1, 1},
+               estr[5] = {1, 1, 1, 1, 1};
+    if (!encode_map(&tmY, y.ptr, 5, dims, strides, box, estr, esz)) return CVVAE_E_CUDA;
+    if (d->residual && !encode_map(&tmR, d->residual, 5, dims, strides, box, estr, esz)) return CVVAE_E_CUDA;
+  }
+
   int rc = CVVAE_OK;
   CVVAE_DISPATCH_DTYPE(d->dtype, {
-    if (N_cta == 256) rc = launch_bn<DT, 256>(tmA, tmB, tmA2, tmB2, p, static_cast<unsigned>(grid), smem, stream);
-    else if (N_cta == 128) rc = launch_bn<DT, 128>(tmA, tmB, tmA2, tmB2, p, static_cast<unsigned>(grid), smem, stream);
-    else rc = launch_bn<DT, 64>(tmA, tmB, tmA2, tmB2, p, static_cast<unsigned>(grid), smem, stream);
+    if (N_cta == 256) rc = launch_bn<DT, 256>(tmA, tmB, tmA2, tmB2, tmY, tmR, p, static_cast<unsigned>(grid), smem, stream);
+    else if (N_cta == 128) rc = launch_bn<DT, 128>(tmA, tmB, tmA2, tmB2, tmY, tmR, p, static_cast<unsigned>(grid), smem, stream);
+    else rc = launch_bn<DT, 64>(tmA, tmB, tmA2, tmB2, tmY, tmR, p, static_cast<unsigned>(grid), smem, stream);
   });
   if (rc != CVVAE_OK) return rc;
   CVVAE_LAUNCH_CHECK();
@@ -876,7 +1092,8 @@ static int conv_tc_plan_query(const cvvae_conv_desc* d, int32_t* out, int32_t n)
                        ok ? p.NA : 0,
                        ok ? p.NB : 0,
                        ok ? static_cast<int32_t>(grid) : 0,
-                       ok ? p.vec2 : 0};
+                       ok ? p.vec2 : 0,
+                       ok ? p.tma_epi : 0};
   constexpr int32_t kFields = static_cast<int32_t>(sizeof(v) / sizeof(v[0]));
   for (int32_t i = 0; i < n && i < kFields; ++i) out[i] = v[i];
   return kFields;

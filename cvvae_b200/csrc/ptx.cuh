@@ -116,6 +116,16 @@ __device__ __forceinline__ uint4 ld_shared_v4(uint32_t addr) {
   asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];\n" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
   return v;
 }
+// No "memory" clobber: global loads around them (bias) may still be batched.  They stay ordered against the other
+// volatile asm (mbarrier waits, proxy fences, barriers) and a load feeds the store of the same word through a register.
+__device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;\n" ::"r"(addr), "r"(v));
+}
+__device__ __forceinline__ uint32_t ld_shared_b32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];\n" : "=r"(v) : "r"(addr));
+  return v;
+}
 
 // ------------------------------------------------------------------ warpgroup MMA
 // Shared-memory matrix descriptor of a K-major operand in SWIZZLE_128B layout: rows of 128 B (64 x 16-bit), 8-row

@@ -167,17 +167,20 @@ class CudaOps:
         return out
 
     @_on_tensor_device
-    def conv_tc_plan(self, x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], **kw) -> dict:
+    def conv_tc_plan(self, x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], *, epilogue: bool = False,
+                     **kw) -> dict:
         """The tile plan ``conv(..., force="tc")`` launches for the same arguments on the current device
         ({name: value} over ``_lib.CONV_TC_PLAN_FIELDS``; ``eligible`` 0 when the tensor-core path refuses them).
-        Launches nothing."""
+        ``epilogue``: also report ``tma_epilogue``, whether the output goes through shared memory and TMA stores
+        (it depends on the output's alignment and on CVVAE_TMA_EPILOGUE, the tiling does not).  Launches nothing."""
         d = self._conv_desc(x, w, bias, **kw)
-        n = len(L.CONV_TC_PLAN_FIELDS)
+        fields = L.CONV_TC_PLAN_EPILOGUE_FIELDS if epilogue else L.CONV_TC_PLAN_FIELDS
+        n = len(fields)
         vals = (C.c_int32 * n)()
         rc = self.lib.cvvae_conv_tc_plan(C.byref(d), vals, n)
         if rc < 0:
             L.check(rc, "cvvae_conv_tc_plan")
-        return dict(zip(L.CONV_TC_PLAN_FIELDS, list(vals)))
+        return dict(zip(fields, list(vals)))
 
     @staticmethod
     def _conv_desc(x, w, bias, *, kernel=(1, 1, 1), stride=(1, 1, 1), offset=(0, 0, 0), pad_t=L.PAD_ZERO, pad_hw=L.PAD_ZERO,

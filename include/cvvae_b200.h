@@ -205,8 +205,10 @@ int cvvae_conv_tc_set_trace(void* device_buf, int32_t n_ctas);
  * int32 values: eligible (0: the tensor-core path refuses it, reason in cvvae_last_error(), every other value 0), N_cta
  * (output channels per CTA), NACC (128-position sub-tiles per CTA), TW, ROWS (= 128/TW), TH (= ROWS*NACC; the patch of
  * one CTA is TH x TW positions, or NACC*128 positions along W when flat), tiles_w, tiles_h, n_tiles_n, flat, NA, NB
- * (activation / weight ring depths), grid (CTAs over all samples), vec2 (channel pairs stored as one word).  Writes
- * the first min(n, count) values and returns count (14), or a negative error code.  Launches nothing. */
+ * (activation / weight ring depths), grid (CTAs over all samples), vec2 (channel pairs stored as one word),
+ * tma_epilogue (the output is staged in shared memory and written by TMA stores, the residual prefetched by TMA; 0 with
+ * CVVAE_TMA_EPILOGUE=0 in the environment).  Writes the first min(n, count) values and returns count (15), or a negative
+ * error code.  Launches nothing. */
 int cvvae_conv_tc_plan(const cvvae_conv_desc* d, int32_t* out, int32_t n);
 const char* cvvae_last_error(void);
 int cvvae_abi_version(void);

@@ -7,6 +7,10 @@ states (bf16: rtol 8e-3).  Integer/data-movement kernels are bit-exact.
 The conv cases here are small: for Cout <= 128 the planner drops them to NACC = 1 sub-tile per CTA, so the branch-free
 wgmma chain and the interior-tile epilogue of the 128- and 64-channel tiles are not reached.  tests/test_gpu_conv_plans.py
 covers those plans, in fp16 and bf16, against an fp64 reference.
+
+These tolerances are wider than one fp16 rounding, so they do not see a truncating store or a one-ulp bias.
+tests/test_gpu_kernels16.py checks the normalisation, softmax, temporal-attention, tap-stacked conv_out and data-movement
+kernels in fp16 and bf16 against fp64 with per-element bounds, a correctly-rounded share and the mean signed ulp error.
 """
 import json
 import os

@@ -64,6 +64,30 @@ class Act:
         self.stats = stats
 
 
+def _phase_fold(w: torch.Tensor, ph: int, pw: int) -> torch.Tensor:
+    """[Co, Ci, 3, 3, 3] -> [Co, Ci, 3, 2, 2]: the 3x3 (H, W) taps of phase (ph, pw) of a nearest-x2 up-sampled input that
+    land on the same input pixel, summed in w's dtype (row 0 alone and rows 1 + 2 for ph = 0; rows 0 + 1 and row 2 for
+    ph = 1; columns alike)."""
+    rows = (w[:, :, :, 0:1], w[:, :, :, 1:2] + w[:, :, :, 2:3]) if ph == 0 else \
+           (w[:, :, :, 0:1] + w[:, :, :, 1:2], w[:, :, :, 2:3])
+    wr = torch.cat(rows, dim=3)  # [Co, Ci, 3, 2, 3]
+    cols = (wr[..., 0:1], wr[..., 1:2] + wr[..., 2:3]) if pw == 0 else \
+           (wr[..., 0:1] + wr[..., 1:2], wr[..., 2:3])
+    return torch.cat(cols, dim=4)
+
+
+def _round_once(w64: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
+    """fp64 -> dtype, rounded once to nearest (ties to even).  A plain cast to a 16-bit type goes through fp32 and can
+    round twice; rounding to fp32 'to odd' (toward zero, then the last bit set when inexact) keeps enough bits for the
+    final rounding to be the correct one."""
+    if dtype not in (torch.float16, torch.bfloat16):
+        return w64.to(dtype)
+    f = w64.float()
+    fd = f.double()
+    t = torch.where(fd.abs() > w64.abs(), torch.nextafter(f, torch.zeros_like(f)), f)
+    return torch.where(fd != w64, (t.view(torch.int32) | 1).view(torch.float32), t).to(dtype)
+
+
 def prepack_params(state_dict: Dict[str, torch.Tensor], ops, dtype: torch.dtype) -> Dict[str, torch.Tensor]:
     """Weights -> [taps, Cout, Cin] in the compute dtype; biases and norm parameters -> fp32."""
     packed = {}
@@ -80,17 +104,18 @@ def prepack_params(state_dict: Dict[str, torch.Tensor], ops, dtype: torch.dtype)
                 # nearest-x2 followed by a 3x3 (H,W) conv == four 2x2 phase convs on the NOT up-sampled input
                 # (exact in real arithmetic): output (2i+ph, 2j+pw) reads input rows {i-1,i} (ph=0) or {i,i+1}
                 # (ph=1) with the taps that land on the same input pixel pre-summed.  2.25x fewer MACs and no
-                # materialised 4x tensor.  Sums are formed in fp32 and rounded once to the compute dtype.
-                w32 = v.float()
+                # materialised 4x tensor.  Sums are formed in fp32 (fp64 for an fp64 model) and rounded once to the
+                # compute dtype.
+                # ".t1": the single-frame form (Engine._single_frame_weights).  The up-sampler's time padding is always
+                # replicate, so on a one-frame input every time tap reads frame 0 and the three time taps of each phase
+                # are summed: twelve checkpoint weights per element, summed exactly in fp64 and rounded once.
+                w32 = v.to(torch.promote_types(v.dtype, torch.float32))
                 for ph in (0, 1):
-                    rows = (w32[:, :, :, 0:1], w32[:, :, :, 1:2] + w32[:, :, :, 2:3]) if ph == 0 else \
-                           (w32[:, :, :, 0:1] + w32[:, :, :, 1:2], w32[:, :, :, 2:3])
-                    wr = torch.cat(rows, dim=3)  # [Co, Ci, 3, 2, 3]
                     for pw in (0, 1):
-                        cols = (wr[..., 0:1], wr[..., 1:2] + wr[..., 2:3]) if pw == 0 else \
-                               (wr[..., 0:1] + wr[..., 1:2], wr[..., 2:3])
-                        wf = torch.cat(cols, dim=4).to(dtype).contiguous()  # [Co, Ci, 3, 2, 2]
-                        packed[k[: -len("weight")] + f"phase{ph}{pw}.weight"] = ops.pack_weight(wf)
+                        key = k[: -len("weight")] + f"phase{ph}{pw}.weight"
+                        packed[key] = ops.pack_weight(_phase_fold(w32, ph, pw).to(dtype).contiguous())
+                        w1 = _round_once(_phase_fold(v.double(), ph, pw).sum(2), dtype)   # [Co, Ci, 2, 2]
+                        packed[key + ".t1"] = ops.pack_weight(w1.contiguous())
                 continue
             packed[k] = ops.pack_weight(v)
             if k in ("encoder.conv_in.weight", "decoder.conv_in.weight") and v.dim() == 5 and tuple(v.shape[3:]) == (3, 3):
@@ -296,8 +321,12 @@ class Engine:
         if key not in self.p:
             w4 = w.view(kt, khw, w.shape[1], w.shape[2])
             if pad_t == PAD_REPLICATE:
-                # one rounding of the fp32 sum, stored like every packed weight ([Co, Ci, khw] -> [khw, Co, Ci])
-                wf = self.ops.pack_weight(w4.float().sum(0).to(w.dtype).permute(1, 2, 0))
+                # the sum of the time taps, rounded once.  An up-sampler phase's stored taps are already rounded sums,
+                # so its fold comes from prepack_params; any other conv stores the checkpoint's taps, summed exactly
+                # here ([Co, Ci, khw] -> [khw, Co, Ci], like every packed weight)
+                wf = self.p.get(wkey + ".t1")
+                if wf is None:
+                    wf = self.ops.pack_weight(_round_once(w4.double().sum(0), w.dtype).permute(1, 2, 0))
             elif 0 <= tl < kt:
                 wf = w4[tl]
             else:

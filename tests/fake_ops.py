@@ -197,7 +197,8 @@ class FakeOps:
         lo_h, lo_w = -offset[0], -offset[1]
         hi_h, hi_w = Ho + kh - 1 - H - lo_h, Wo + kw - 1 - W - lo_w
         xin = _ncdhw(x)
-        xin = F.pad(xin.float(), (lo_w, hi_w, lo_h, hi_h, 0, 0), mode="replicate" if pad_hw == PAD_REPLICATE else "constant").to(x.dtype)
+        xin = F.pad(xin.to(torch.promote_types(x.dtype, torch.float32)), (lo_w, hi_w, lo_h, hi_h, 0, 0),
+                    mode="replicate" if pad_hw == PAD_REPLICATE else "constant").to(x.dtype)
         out.zero_()
         for a in range(kh):
             for b in range(kw):

@@ -11,6 +11,8 @@ covers those plans, in fp16 and bf16, against an fp64 reference.
 These tolerances are wider than one fp16 rounding, so they do not see a truncating store or a one-ulp bias.
 tests/test_gpu_kernels16.py checks the normalisation, softmax, temporal-attention, tap-stacked conv_out and data-movement
 kernels in fp16 and bf16 against fp64 with per-element bounds, a correctly-rounded share and the mean signed ulp error.
+tests/test_gpu_attention16.py does the same for the three attention GEMMs, the softmax hand-off and the whole spatial
+attention at the tiler's token counts (the two attention tests here run at N = 1024 and 200, fp16 only).
 """
 import json
 import os

@@ -10,7 +10,8 @@ of the open chunk in a staging buffer of S+1 frames, run each chunk through ``mo
 chunk however long the clip is, and the concatenated chunks are bit-identical to the whole-clip call.
 
 ``reconstruct_frames`` chains pixel upload, encoder, posterior, decoder and pixel download over host uint8 frames:
-the body of the reference's ``cvvae_inference_video.py`` as a stream.
+the body of the reference's ``cvvae_inference_video.py`` as a stream.  ``evaluate_frames`` is the same stream with every
+reconstructed frame scored (PSNR, SSIM) on the device against the input frame the network saw.
 """
 from __future__ import annotations
 
@@ -158,17 +159,43 @@ def reconstruct_frames(model, frames: Iterable, size=None, sample_posterior: boo
     memory holds about one chunk.  Yielded tensors are the caller's: later pieces never overwrite them.  Only float16
     and bfloat16 models are supported (the pixel conversion kernels are 16-bit).
     """
+    enc, dec = _open(model, "reconstruct_frames")
+    return _reconstruct(model, enc, dec, iter(frames), size, sample_posterior, generator, False)
+
+
+def evaluate_frames(model, frames: Iterable, size=None, sample_posterior: bool = False,
+                    generator: Optional[torch.Generator] = None) -> Iterator[tuple]:
+    """``reconstruct_frames`` with a score for every frame: yields ``(frames_u8, psnr, ssim)`` per piece.
+
+    Same inputs and refusals as ``reconstruct_frames``, and ``frames_u8`` is what it yields.  ``psnr`` and ``ssim`` are
+    float64 host tensors with one entry per frame of the piece (``cvvae_b200.metrics`` has the definitions).  Output
+    frame i is scored against input frame i as the network saw it: after the resize to `size`, as uint8, before
+    ``/ 127.5 - 1``.  The trailing frames past ``1 + (T-1)//4*4`` are not reconstructed and so not scored.
+    The networks reproduce frame sizes that are a multiple of their spatial stride; when the reconstruction's size differs
+    from the input's there is nothing to score it against and ``ValueError`` is raised: pass such a `size`.
+
+    The scores are computed on the device, one kernel per piece right after the pixel conversion, and travel to the
+    host with the frames.  The uint8 input of a chunk stays on the device until its reconstruction appears, so the
+    stream holds at most two chunks' uint8 frames more than ``reconstruct_frames``, whatever the clip's length.
+    """
+    enc, dec = _open(model, "evaluate_frames")
+    return _reconstruct(model, enc, dec, iter(frames), size, sample_posterior, generator, True)
+
+
+def _open(model, who: str):
     if model.dtype not in (torch.float16, torch.bfloat16):
-        raise ValueError(f"reconstruct_frames: the pixel conversion is float16 / bfloat16 only; model dtype is {model.dtype}")
+        raise ValueError(f"{who}: the pixel conversion is float16 / bfloat16 only; model dtype is {model.dtype}")
     if model.device.type != "cuda":
-        raise ValueError("reconstruct_frames: the model must be on a CUDA device")
-    enc, dec = StreamEncoder(model), StreamDecoder(model)   # raise for models without temporal chunking
-    return _reconstruct(model, enc, dec, iter(frames), size, sample_posterior, generator)
+        raise ValueError(f"{who}: the model must be on a CUDA device")
+    return StreamEncoder(model), StreamDecoder(model)   # raise for models without temporal chunking
 
 
 def _reconstruct(model, enc: StreamEncoder, dec: StreamDecoder, frames: Iterator, size, sample_posterior: bool,
-                 generator) -> Iterator[torch.Tensor]:
-    from .video_io import frames_to_input, output_to_frames
+                 generator, score: bool) -> Iterator:
+    """The stream behind reconstruct_frames (`score` False: yields frames) and evaluate_frames (True: yields
+    (frames, psnr, ssim))."""
+    from . import metrics
+    from .video_io import frames_to_input, frames_to_input_and_u8, output_to_frames
 
     # No device context is held across the yields (it would leak into the caller's code): every allocation, stream and
     # launch below names the model's device, and the networks run on that device's current stream.
@@ -178,19 +205,53 @@ def _reconstruct(model, enc: StreamEncoder, dec: StreamDecoder, frames: Iterator
     staging: Optional[torch.Tensor] = None   # pinned upload buffer, refilled once its last upload has completed
     staged = torch.cuda.Event()
     pending: deque = deque()    # input frames on the device, not yet fed: the clip may end before they are kept
+    refs: deque = deque()       # score only: uint8 input frames as the network saw them, from the first frame not yet scored
     fed = received = 0
-    downloads: deque = deque()  # (host frames, event of their download), oldest first
+    downloads: deque = deque()  # (host frames, host int64 sums of their scores or None, event of their download), oldest first
+
+    def take_refs(n: int) -> torch.Tensor:
+        """The next `n` input frames: decoder chunks return the clip's frames in order, [0, 17) then 16 at a time."""
+        parts = []
+        while n:
+            r = refs.popleft()
+            if r.shape[0] > n:
+                refs.appendleft(r[n:])
+                r = r[:n]
+            parts.append(r)
+            n -= r.shape[0]
+        return parts[0] if len(parts) == 1 else torch.cat(parts)
 
     def download(x: torch.Tensor) -> None:
         u8 = output_to_frames(x)
         host = _pinned(u8.shape, u8)
+        acc = None
+        if score:
+            ref = take_refs(u8.shape[0])
+            if ref.shape != u8.shape:
+                raise ValueError(f"evaluate_frames: the networks return {u8.shape[1]} x {u8.shape[2]} frames for an input of "
+                                 f"{ref.shape[1]} x {ref.shape[2]}, and frames of different sizes cannot be scored; pass "
+                                 "`size=` with a size the networks reproduce (a multiple of their spatial stride)")
+            acc = metrics._launch(ref, u8)
+        sums = _pinned(acc.shape, acc) if score else None
         copy.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(copy):
             host.copy_(u8, non_blocking=True)
+            if score:
+                sums.copy_(acc, non_blocking=True)
             done = torch.cuda.Event()
             done.record(copy)
         u8.record_stream(copy)
-        downloads.append((host, done))
+        if score:
+            acc.record_stream(copy)
+        downloads.append((host, sums, done))
+
+    def piece():
+        host, sums, done = downloads.popleft()
+        done.synchronize()
+        if not score:
+            return host
+        m = metrics._scores(sums, host.shape[1], host.shape[2])
+        return host, m.psnr, m.ssim
 
     def decode_chunks(latent_chunks) -> None:
         for post in latent_chunks:
@@ -201,8 +262,8 @@ def _reconstruct(model, enc: StreamEncoder, dec: StreamDecoder, frames: Iterator
     for item in frames:
         item = torch.as_tensor(item)
         if item.dtype != torch.uint8 or item.dim() != 4 or item.shape[-1] != 3 or item.device.type != "cpu":
-            raise ValueError(f"reconstruct_frames expects host uint8 frames [t, H, W, 3]; got {item.dtype} "
-                             f"{tuple(item.shape)} on {item.device}")
+            raise ValueError(f"{'evaluate_frames' if score else 'reconstruct_frames'} expects host uint8 frames "
+                             f"[t, H, W, 3]; got {item.dtype} {tuple(item.shape)} on {item.device}")
         t = item.shape[0]
         if t == 0:
             continue
@@ -218,7 +279,12 @@ def _reconstruct(model, enc: StreamEncoder, dec: StreamDecoder, frames: Iterator
         compute = torch.cuda.current_stream(dev)
         compute.wait_event(staged)
         dev_u8.record_stream(compute)
-        pending.append(frames_to_input(dev_u8, dtype=model.dtype, size=size))
+        if score:
+            x, ref = frames_to_input_and_u8(dev_u8, dtype=model.dtype, size=size)
+            pending.append(x)
+            refs.append(ref)
+        else:
+            pending.append(frames_to_input(dev_u8, dtype=model.dtype, size=size))
         received += t
         # feed up to the last frame the script keeps so far (1 + (T-1)//4*4): frames past it wait for more input, and
         # are dropped if the clip ends first
@@ -232,14 +298,11 @@ def _reconstruct(model, enc: StreamEncoder, dec: StreamDecoder, frames: Iterator
             fed += k
         # one-chunk lag: a piece goes to the caller only once a later chunk is enqueued behind it
         while len(downloads) > 1:
-            host, done = downloads.popleft()
-            done.synchronize()
-            yield host
+            yield piece()
     pending.clear()
     decode_chunks(enc.close())
     for x in dec.close():
         download(x)
+    refs.clear()   # the trailing frames that were never reconstructed
     while downloads:
-        host, done = downloads.popleft()
-        done.synchronize()
-        yield host
+        yield piece()

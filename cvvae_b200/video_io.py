@@ -37,19 +37,31 @@ def resize_frames(frames_u8: torch.Tensor, size) -> torch.Tensor:
 def frames_to_input(frames_u8: torch.Tensor, dtype: torch.dtype = torch.float16, size=None) -> torch.Tensor:
     """uint8 [T, H, W, 3] on the GPU -> [1, 3, T, H, W] in [-1, 1]; with `size=(h, w)` the frames are resized first
     (one fused pass: resize -> round to uint8 -> `.half() / 127.5 - 1.0`)."""
+    return _to_input(frames_u8, dtype, size, False)[0]
+
+
+def frames_to_input_and_u8(frames_u8: torch.Tensor, dtype: torch.dtype = torch.float16, size=None):
+    """`frames_to_input` plus the uint8 frames the result was computed from, [T, h, w, 3]: the resized frames, written by
+    the same launch, or `frames_u8` itself when nothing is resized."""
+    return _to_input(frames_u8, dtype, size, True)
+
+
+def _to_input(frames_u8: torch.Tensor, dtype: torch.dtype, size, want_u8: bool):
     frames_u8 = _check_frames(frames_u8, "frames_to_input")
     T, H, W, _ = frames_u8.shape
     if size is not None and (int(size[0]), int(size[1])) != (H, W):
         oh, ow = int(size[0]), int(size[1])
         out = torch.empty((1, 3, T, oh, ow), dtype=dtype, device=frames_u8.device)
+        u8 = torch.empty((T, oh, ow, 3), dtype=torch.uint8, device=frames_u8.device) if want_u8 else None
         with torch.cuda.device(frames_u8.device):
-            L.check(L.load().cvvae_video_resize_u8(frames_u8.data_ptr(), None, out.data_ptr(), T, H, W, oh, ow, dtype_code(dtype),
+            L.check(L.load().cvvae_video_resize_u8(frames_u8.data_ptr(), u8.data_ptr() if want_u8 else None, out.data_ptr(),
+                                                   T, H, W, oh, ow, dtype_code(dtype),
                                                    torch.cuda.current_stream(out.device).cuda_stream), "cvvae_video_resize_u8")
-        return out
+        return out, u8
     out = torch.empty((1, 3, T, H, W), dtype=dtype, device=frames_u8.device)
     L.check(L.load().cvvae_video_u8_to_f16(frames_u8.data_ptr(), out.data_ptr(), T, H, W, dtype_code(dtype),
                                            torch.cuda.current_stream(out.device).cuda_stream), "cvvae_video_u8_to_f16")
-    return out
+    return out, frames_u8
 
 
 def output_to_frames(x: torch.Tensor) -> torch.Tensor:

@@ -196,6 +196,22 @@ int cvvae_video_f16_to_u8(const void* in_cthw, uint8_t* thwc, int32_t T, int32_t
 int cvvae_video_resize_u8(const uint8_t* thwc, uint8_t* out_thwc, void* out_cthw, int32_t T, int32_t H, int32_t W, int32_t OH,
                           int32_t OW, int32_t dtype, void* stream);
 
+/* Reconstruction quality: per-frame squared error and SSIM of two uint8 videos a, b: [T,H,W,3], contiguous, on the device.
+ * They are the two ends of the inference script: its resized uint8 input (cvvae_inference_video.py:28) and the uint8
+ * frames it writes (:47-50).
+ *   acc: int64 [T][2], overwritten:  acc[t][0] = sum over (h,w,c) of (a-b)^2, the whole frame (exact)
+ *                                    acc[t][1] = sum over the valid (h,w,c) of llrint(ssim * 2^32)
+ * SSIM (Wang et al. 2004): per colour channel, at every (y,x) with 5 <= y < H-5, 5 <= x < W-5 (no padding), under the window
+ * w = g (x) g, g = the 11-tap Gaussian exp(-k^2 / (2 * 1.5^2)) normalised to sum 1: means mu_a, mu_b, variances and
+ * covariance E[a^2] - mu_a^2, E[b^2] - mu_b^2, E[ab] - mu_a mu_b; C1 = (0.01 * 255)^2, C2 = (0.03 * 255)^2;
+ *   ssim = (2 mu_a mu_b + C1)(2 s_ab + C2) / ((mu_a^2 + mu_b^2 + C1)(s_a^2 + s_b^2 + C2)).
+ * Frame SSIM = acc[t][1] / 2^32 / (3 (H-10) (W-10)); PSNR = 10 log10(255^2 * 3 H W / acc[t][0]).  The moments are exact
+ * integer sums along rows and fp64 along columns, the formula is fp32; identical frames give exactly 2^32 per position.
+ * Integer accumulation: bit-reproducible and independent of how the frames are split over calls.
+ * T >= 0 (T == 0 launches nothing), H, W >= 11 and 3*H*W < 2^31, else CVVAE_E_ARG.  One kernel launch. */
+int cvvae_frame_metrics(const uint8_t* a_thwc, const uint8_t* b_thwc, int32_t T, int32_t H, int32_t W, int64_t* acc,
+                        void* stream);
+
 /* Diagnostics */
 /* Per-CTA phase timestamps of the next conv_tc launches: device buffer of n_ctas x 8 uint64 (globaltimer ns:
  * entry, setup done, first A landed, first B landed, all MMAs issued, accumulators ready, epilogue done,

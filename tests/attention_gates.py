@@ -162,7 +162,11 @@ def stats_gate(y, st, groups):
     """Gate 5 of test_gpu_conv_plans.py: fused statistics st [B, groups, 2] (fixed point) against fp64 sums of the
     stored y [B, ..., C].  Returns (max abs error, [failures])."""
     v = y.double().reshape(y.shape[0], -1, groups, y.shape[-1] // groups)
-    want = torch.stack([v.sum(dim=(1, 3)), (v * v).sum(dim=(1, 3))], dim=-1)
+    return stats_compare(torch.stack([v.sum(dim=(1, 3)), (v * v).sum(dim=(1, 3))], dim=-1), st)
+
+
+def stats_compare(want, st):
+    """stats_gate against sums computed by the caller: want [B, groups, 2] (fp64 sum, sum of squares)."""
     got = torch.stack([st[..., 0].double() / GN_SUM_SCALE, st[..., 1].double() / GN_SQ_SCALE], dim=-1)
     try:
         torch.testing.assert_close(got, want, rtol=1e-5, atol=2e-2)

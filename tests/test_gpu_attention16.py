@@ -30,6 +30,7 @@ import pytest
 import torch
 
 import attention_gates as AG
+import kernel_bounds as KB
 import test_gpu_ops
 from cvvae_b200.engine import Engine, NetConfig, _round_once
 from test_gpu_upsample16 import _Recording
@@ -358,7 +359,6 @@ def _run_block(variant, attn_type, p, params, x, dtype):
 def test_attention_block16(name, dt, monkeypatch):
     """Every launch of the block replayed against its spec in fp64 on its recorded inputs; proj_out's fused statistics
     (flat plan, residual, TMA epilogue) against fp64 sums and bit for bit against the register epilogue."""
-    import test_gpu_kernels16 as K16
     variant, attn_type, p, (H, W), T = BLOCK_CASES[name]
     dtype, C, G = DTYPES[dt], BLOCK_C, 32
     torch.cuda.reset_peak_memory_stats()
@@ -383,27 +383,18 @@ def test_attention_block16(name, dt, monkeypatch):
         if kind == "groupnorm":
             xi, gam, bet, groups, eps, kw = args
             assert kw == dict(per_frame=True, silu=False), kw
-            pix, ppb, lanes, nblocks, _ = K16._gn_geometry(tuple(xi.shape), True)
+            pix, ppb, lanes, nblocks, _ = KB.gn_geometry(tuple(xi.shape), True)
             assert pix == N and nblocks > 1, (pix, nblocks)
-            cpg = C // groups
-            eps_sum = (-(-ppb // lanes) + 7) * K16.U32
-            fix = nblocks * lanes * -(-cpg // 8) / (pix * cpg)
-            r, E, _ = K16._gn_reference(xi, gam, bet, groups, eps, True, False, eps_sum, fix)
+            eps_sum, fix, _ = KB.gn_sum_terms(tuple(xi.shape), True, groups)
+            r, E, _ = KB.gn_reference(xi, gam, bet, groups, eps, True, False, eps_sum, fix)
             gt = AG.Gates(dtype).add(y, r, E)
         elif kind == "layernorm":
             xi, gam, bet, eps = args
-            xd = xi.double()
-            z = (xd - xd.mean(-1, keepdim=True)) / torch.sqrt(xd.var(-1, unbiased=False, keepdim=True) + eps)
-            r = z * gam.double() + bet.double()
-            gt = AG.Gates(dtype).add(y, r, 2.0 ** -16 * (gam.double().abs() * (1 + z.abs()) + bet.double().abs()))
+            r, E, rec["layernorm_max_mean_over_std"] = KB.layernorm_reference(xi, gam, bet, eps)
+            gt = AG.Gates(dtype).add(y, r, E)
         else:
-            qd, kd, vd = (t.double().permute(0, 2, 3, 1, 4).reshape(H * W, T, C) for t in args)
-            a = torch.softmax(qd @ kd.transpose(1, 2) * C ** -0.5, dim=-1)
-            A = ((qd.abs() @ kd.abs().transpose(1, 2)) * C ** -0.5).amax(-1, keepdim=True)
-            n1 = 8 * -(-C // 256)
-            E = K16.U32 * ((2 * n1 + 19) * A + 2 * T + 5) * (a @ vd.abs())
-            back = lambda t: t.reshape(1, H, W, T, C).permute(0, 3, 1, 2, 4)
-            gt = AG.Gates(dtype).add(y, back(a @ vd), back(E))
+            r, E, _ = KB.attn_temporal_reference(*args)
+            gt = AG.Gates(dtype).add(y, r, E)
         rec[kind], f_k = gt.result()
         failed += [f"{kind} {f}" for f in f_k]
 

@@ -28,28 +28,16 @@ import torch
 import torch.nn.functional as F
 
 import block_cases as BC
+import kernel_bounds as KB
 import test_gpu_conv_plans as CP
 import test_gpu_ops
 from fake_ops import PAD_REPLICATE, PAD_ZERO, FakeOps
-from test_gpu_fp32 import _ulp as _ulp_p
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
 OUT = test_gpu_ops.OUT
 DTYPES = {"fp16": torch.float16, "bf16": torch.bfloat16}
-U32 = 2.0 ** -24   # unit roundoff of fp32
-
-# Gate 2.  The kernel's fp32 value c is within E of r, so it rounds to a different 16-bit number than r only when a
-# rounding midpoint lies between them: for r placed at random on the 16-bit grid that happens with probability
-# |c - r| / ulp <= E / ulp.  mean(min(1, E / ulp)) therefore over-estimates the mismatch rate (E is a worst case); the
-# margin covers the sampling noise of cases with few elements.  A truncating store mismatches ~50 %.  Where E is far
-# above the typical error (a sum of n roundings is typically sqrt(n) times below its bound: conv_stacked's 58-term
-# bound puts the estimate at 0.3-0.45 for fp16), the estimate says little, so the gate never asks for less than
-# SHARE_FLOOR, which a truncating store still misses by half.
-MISMATCH_MARGIN = 2.0
-SHARE_FLOOR = 0.75
-# Gate 3.  Correct rounding has mean signed error ~0 +- 0.3 / sqrt(n) ulp; directed rounding gives +-0.5 ulp.
-MAX_MEAN_ULP = 0.05
+U32 = KB.U32
 _RECORD = {}
 
 
@@ -63,11 +51,6 @@ def _rand(shape, dtype, seed, scale=1.0, offset=0.0):
     return ((torch.rand(shape, generator=g, dtype=torch.float64) * 2 - 1) * scale + offset).to(dtype).to(DEV)
 
 
-def _ulp(r, dtype):
-    """Spacing of `dtype` numbers at |r| (r float64), from the exponent bits (test_gpu_fp32._ulp)."""
-    return _ulp_p(r, 11, -14) if dtype == torch.float16 else _ulp_p(r, 8, -126)
-
-
 def _dump():
     os.makedirs(OUT, exist_ok=True)
     with open(os.path.join(OUT, "kernels16.json"), "w") as f:
@@ -75,87 +58,15 @@ def _dump():
 
 
 def _gates(tag, y, r, E, dtype, **extra):
-    """Gates 1-3 on a 16-bit result y against its fp64 reference r and fp32 error bound E; records, returns failures."""
-    yd = y.double()
-    ulp = _ulp(r, dtype)
-    err = yd - r
-    ratio = (err.abs() / (0.5 * ulp + E)).max().item()
-    rn = torch.round(r / ulp) * ulp                     # r / ulp is exact in fp64; round half to even
-    share = (yd == rn).double().mean().item()
-    est = (E / ulp).clamp(max=1.0).mean().item()
-    min_share = max(1.0 - MISMATCH_MARGIN * est, SHARE_FLOOR)
-    mean_ulp = (err / ulp).mean().item()
-    failed = []
-    if not ratio <= 1.0:
-        failed.append(f"1: |y - r| exceeds the bound by {ratio:.3f}x")
-    if not share >= min_share:
-        failed.append(f"2: {share:.4f} correctly rounded < {min_share:.4f}")
-    if not abs(mean_ulp) <= MAX_MEAN_ULP:
-        failed.append(f"3: mean signed error {mean_ulp:+.4f} ulp")
-    _RECORD[tag] = {"numel": y.numel(), "worst_bound_ratio": ratio, "correctly_rounded_share": share,
-                    "mismatch_est": est, "min_share": min_share, "mean_signed_ulp": mean_ulp, "failed_gates": failed, **extra}
+    """Gates 1-3 (kernel_bounds._gates) on a 16-bit result; records under `tag`, returns the failures."""
+    rec, failed = KB._gates(y, r, E, dtype)
+    _RECORD[tag] = {**rec, **extra}
     _dump()
     return [f"{tag}: {f}" for f in failed]
 
 
 # ------------------------------------------------------------------------------------------------------------ GroupNorm
-# Statistics pass (gn_stats_kernel): each thread sums its 8 channels over P_t = ceil(ppb / lanes) positions in fp32
-# (lanes = 256 / (C / 8) positions per sweep, ppb positions per CTA: pick_grid), then folds min(cpg, 8) channel sums into
-# each of its groups; the square of a 16-bit value is exact in fp32.  Recursive summation of n terms is off by at most
-# n u sum|x_i|, so with eps_sum = (P_t + 7) u the sums are off by eps_sum sum|x| and eps_sum sum x^2.  Each partial is then
-# rounded to the fixed point (1/2 * 2^-20 for the sum, 1/2 * 2^-18 for the squares); a group receives nblocks * lanes *
-# ceil(cpg / 8) partials, N_c per element (fix below).  The block and device sums are exact integers, and the apply
-# kernel turns them into mean and variance in fp64:
-#     dm   = eps_sum E|x|  + 2^-21 N_c            dsq = eps_sum E[x^2] + 2^-19 N_c
-#     var  = E[x^2] - mean^2  ->  dvar = dsq + 2 |mean| dm + dm^2
-#     z = (x - mean) rstd     ->  dz   = 1/2 dvar / (var + eps) |z| (1.01: second order) + dm rstd
-# For an input whose mean is k standard deviations, dvar ~ eps_sum sigma^2 (1 + k^2 + 2 k sqrt(1 + k^2)) ~ 3 k^2 eps_sum
-# sigma^2: z is off by ~1.5 k^2 eps_sum |z|, 2^-14 |z| at k = 5 and C = 128 (P_t = 16): the large-mean case checks it.
-# Statistics handed in through stats= (exact fp64 sums rounded once to the fixed point): dm = 2^-21 / cnt,
-# dsq = 2^-19 / cnt.
-# The apply kernel rounds rstd and mean to fp32, forms a = rstd gamma and b = beta - mean a in fp32 and stores
-# fma(x, a, b): at most 6 roundings of terms of size |gamma| (|z| + k) or |beta| + |gamma| k, under
-# 2^-21 (|gamma| (|z| + 2k + 1) + |beta|).  SiLU has slope in [-0.1, 1.1] and __expf / __fdividef / the add cost under
-# 2^-18 |y| for |pre| <= 10.  E = |gamma| dz + 2^-21 (...), times 1.1 plus 2^-18 |r| with SiLU; then the 16-bit store.
-def _gn_reference(x, gamma, beta, G, eps, per_frame, silu, eps_sum, fix):
-    B, T, H, W, Cc = x.shape
-    cpg = Cc // G
-    xd = x.double()
-    v = xd.reshape(B * T, H * W, G, cpg) if per_frame else xd.reshape(B, T * H * W, G, cpg)
-    mean = v.mean(dim=(1, 3), keepdim=True)
-    var = v.var(dim=(1, 3), unbiased=False, keepdim=True)
-    sd = torch.sqrt(var + eps)
-    z = (v - mean) / sd
-    if eps_sum is None:                                    # exact statistics through stats=
-        cnt = v.shape[1] * cpg
-        dm, dsq = 2.0 ** -21 / cnt, 2.0 ** -19 / cnt
-    else:
-        dm = eps_sum * v.abs().mean(dim=(1, 3), keepdim=True) + 2.0 ** -21 * fix
-        dsq = eps_sum * (v * v).mean(dim=(1, 3), keepdim=True) + 2.0 ** -19 * fix
-    dvar = dsq + 2 * mean.abs() * dm + dm * dm
-    k = mean.abs() / sd
-    dz = 0.5 * 1.01 * dvar / (var + eps) * z.abs() + dm / sd
-    gam = gamma.double().view(1, 1, G, cpg)
-    bet = beta.double().view(1, 1, G, cpg)
-    pre = z * gam + bet
-    E = gam.abs() * dz + 2.0 ** -21 * (gam.abs() * (z.abs() + 2 * k + 1) + bet.abs())
-    r = pre
-    if silu:
-        r = pre * torch.sigmoid(pre)
-        E = 1.1 * E + 2.0 ** -18 * r.abs()
-    return r.reshape(x.shape), E.reshape(x.shape), k.max().item()
-
-
-def _gn_geometry(shape, per_frame):
-    """pick_grid / gn_*_kernel: positions per CTA, positions per sweep, CTAs, positions in the last CTA."""
-    B, T, H, W, Cc = shape
-    pix = H * W if per_frame else T * H * W
-    ppb = max(256, -(-pix // 1184))
-    lanes = 256 // (Cc // 8)
-    nblocks = -(-pix // ppb)
-    return pix, ppb, lanes, nblocks, pix - (nblocks - 1) * ppb
-
-
+# The statistics and apply kernels' bound: kernel_bounds.gn_pointwise.
 # name: (shape [B,T,H,W,C], per_frame, silu, layout, offset of the input's mean); C in {64, 128, 256, 512} with 32 groups
 GN_CASES = {
     "c64_cpg2": ((1, 5, 24, 20, 64), False, True, "dense", 0.3),
@@ -178,7 +89,7 @@ def test_groupnorm16(name, dt):
     G, eps = 32, 1e-6
     cpg = Cc // G
     # the case reaches the branches it is named for
-    pix, ppb, lanes, nblocks, n_last = _gn_geometry(shape, per_frame)
+    pix, ppb, lanes, nblocks, n_last = KB.gn_geometry(shape, per_frame)
     assert n_last % (4 * lanes) != 0, "positions of the last CTA leave no tail after the 4-way unrolled loop"
     assert name.split("_")[1] == f"cpg{cpg}" and ((cpg < 8) == (Cc < 256))
     scale = 1.0 if offset > 1 else 2.0
@@ -193,10 +104,9 @@ def test_groupnorm16(name, dt):
     failed = []
 
     # statistics computed by the kernel
-    eps_sum = (-(-ppb // lanes) + 7) * U32
-    fix = nblocks * lanes * -(-cpg // 8) / (pix * cpg)
+    eps_sum, fix, _ = KB.gn_sum_terms(shape, per_frame, G)
     y = ops.groupnorm(x, gam, bet, G, eps, per_frame=per_frame, silu=silu)
-    r, E, k = _gn_reference(x, gam, bet, G, eps, per_frame, silu, eps_sum, fix)
+    r, E, k = KB.gn_reference(x, gam, bet, G, eps, per_frame, silu, eps_sum, fix)
     if offset > 1:
         assert k > 4.0, k                                   # mean several standard deviations from zero
     failed += _gates(f"groupnorm/{name}/kernel_stats/{dt}", y, r, E, dtype, max_mean_over_std=k, eps_sum=eps_sum)
@@ -208,7 +118,7 @@ def test_groupnorm16(name, dt):
         st[..., 0] = torch.round(v.sum(dim=(1, 3)) * 2.0 ** 20).long()
         st[..., 1] = torch.round((v * v).sum(dim=(1, 3)) * 2.0 ** 18).long()
         y2 = ops.groupnorm(x, gam, bet, G, eps, per_frame=False, silu=silu, stats=st)
-        r2, E2, _ = _gn_reference(x, gam, bet, G, eps, False, silu, None, None)
+        r2, E2, _ = KB.gn_reference(x, gam, bet, G, eps, False, silu, None, None)
         failed += _gates(f"groupnorm/{name}/exact_stats/{dt}", y2, r2, E2, dtype)
 
     # framed output (SD3 conv_norm_out): the interior equals the dense result bit for bit, the frame replicates it
@@ -223,10 +133,7 @@ def test_groupnorm16(name, dt):
 
 
 # ------------------------------------------------------------------------------------------------------------ LayerNorm
-# One warp per token, two-pass fp32 statistics: the sum over C is off by (C / 32 + 5) u sum|x|, mean = sum / C exact (C a
-# power of two), the squared deviations by (C / 32 + 7) u, rsqrtf 2 ulp, then (x - mean) rstd gamma + beta in <= 4
-# roundings: for inputs with |mean| <= sigma, E <= 2^-19 (|gamma| (1 + |z|) + |beta|).  The fp32 form of
-# test_gpu_fp32._norm_bound, 2^-16 (|gamma| (1 + |z|) + |beta|), covers it.
+# Bound: kernel_bounds.layernorm_reference (|mean| <= sigma here: the 2^-16 (|gamma| (1 + |z|) + |beta|) form).
 @pytest.mark.parametrize("dt", sorted(DTYPES))
 @pytest.mark.parametrize("shape", [(2, 3, 5, 7, 512), (1, 3, 7, 9, 128)])
 def test_layernorm16(shape, dt):
@@ -237,18 +144,13 @@ def test_layernorm16(shape, dt):
     gam = _rand((Cc,), torch.float32, 31, 0.5, 1.0)
     bet = _rand((Cc,), torch.float32, 32, 0.2)
     y = ops.layernorm(x, gam, bet, 1e-5)
-    xd = x.double()
-    z = (xd - xd.mean(-1, keepdim=True)) / torch.sqrt(xd.var(-1, unbiased=False, keepdim=True) + 1e-5)
-    r = z * gam.double() + bet.double()
-    E = 2.0 ** -16 * (gam.double().abs() * (1 + z.abs()) + bet.double().abs())
+    r, E, _ = KB.layernorm_reference(x, gam, bet, 1e-5)
     failed = _gates(f"layernorm/C{Cc}/{dt}", y, r, E, dtype)
     assert not failed, "; ".join(failed)
 
 
 # ---------------------------------------------------------------------------------------------------------- softmax_rows
-# test_gpu_fp32's softmax bound: __expf(s - m) is within 2^-22 + 2.5 u |s - m| relative; the row sum adds at most
-# cols / 1024 + 2 (vector path) or cols / 256 (scalar path) terms per thread plus 13 in the warp and block reductions, under
-# 92 u = 2^-17.5 at 20 000 columns; 1 / sum and the product two more roundings:  E = 2^-18 r (4 + |s - m|).
+# Bound: kernel_bounds.softmax_reference, E = 2^-18 r (4 + |s - m|).
 # Gate 3 in fp16 at 20 000 columns: 17 % of the probabilities lie below half the subnormal spacing, and within each ulp
 # step they are denser toward zero, so r rounded once is itself off by -0.025 ulp on average (-0.008 at 5184 columns).
 # name: (rows, cols, ld_s, ld_p, misaligned).  1024 / 4096 / 5184: mid-block tokens of 256- / 512- / 576-px tiles.
@@ -283,9 +185,7 @@ def test_softmax_rows16(name, dt):
         assert cols > 12288 and 4 * cols > 48 * 1024, "the row fits the default 48 KB of shared memory"
     ops.softmax_rows(s, cols, p)
     torch.cuda.synchronize()
-    sd = s[:, :cols].double()
-    r = torch.softmax(sd, dim=-1)
-    E = 2.0 ** -18 * r * (4 + (sd - sd.max(-1, keepdim=True).values).abs())
+    r, E = KB.softmax_reference(s, cols)
     failed = _gates(f"softmax_rows/{name}/{dt}", p[:, :cols], r, E, dtype)
     # columns between cols and ld, and the buffer outside the rows, are left untouched
     untouched = torch.cat([p[:, cols:].flatten(), p_buf[:o], p_buf[o + rows * ld_p:]])
@@ -294,12 +194,7 @@ def test_softmax_rows16(name, dt):
 
 
 # -------------------------------------------------------------------------------------------------- temporal attention
-# One warp per position, fp32 throughout.  Scores: each lane adds n1 = 8 ceil(C / 256) products, then 5 shuffle adds, the
-# scale and its own rounding: |ds| <= (n1 + 7) u A_i, A_i = max_j C^-0.5 sum_c |q_ic k_jc|.  A probability is off by
-# 2 |ds| (its score and the max), 2.5 u |s - m| <= 5 u A_i (subtraction, __expf's argument scaling), 2^-22 (ex2.approx),
-# (T - 1) u (the sum over T) and 2 u (1 / sum, the product); the value sum is an fma chain over T frames, T u sum p |v|:
-#     E = u ((2 n1 + 19) A_i + 2 T + 5) sum_j p_ij |v_j|.
-# At T = 5, C = 512 this is the fp32 file's 2^-16 (1 + A_i) sum p |v| to within 20 %; it grows with T.
+# Bound: kernel_bounds.attn_temporal_reference, E = u ((2 n1 + 19) A_i + 2 T + 5) sum_j p_ij |v_j|.
 # name: (shape [B,T,H,W,C], MAXT of the instantiation that runs it)
 ATTN_CASES = {
     "T5_C512": ((1, 5, 3, 5, 512), 32),
@@ -323,23 +218,14 @@ def test_attn_temporal16(name, dt):
     q, k = (_rand(shape, dtype, 34 + i, s) for i in range(2))
     v = _rand(shape, dtype, 36, 1.0, 0.5)
     o = ops.attn_temporal(q, k, v)
-    qd, kd, vd = (t.double().permute(0, 2, 3, 1, 4).reshape(B * H * W, T, Cc) for t in (q, k, v))
-    a = torch.softmax(qd @ kd.transpose(1, 2) * Cc ** -0.5, dim=-1)
-    pmax = a.amax(-1).mean().item()
+    r, E, pmax = KB.attn_temporal_reference(q, k, v)
     assert 2.0 / T < pmax < 0.9, f"softmax is flat or one-hot (mean max p {pmax:.3f})"
-    A = ((qd.abs() @ kd.abs().transpose(1, 2)) * Cc ** -0.5).amax(-1, keepdim=True)
-    n1 = 8 * -(-Cc // 256)
-    E = U32 * ((2 * n1 + 19) * A + 2 * T + 5) * (a @ vd.abs())
-    back = lambda t: t.reshape(B, H, W, T, Cc).permute(0, 3, 1, 2, 4)
-    failed = _gates(f"attn_temporal/{name}/{dt}", o, back(a @ vd), back(E), dtype, mean_max_p=pmax)
+    failed = _gates(f"attn_temporal/{name}/{dt}", o, r, E, dtype, mean_max_p=pmax)
     assert not failed, "; ".join(failed)
 
 
 # ------------------------------------------------------------------------------------------ tap-stacked conv_out kernel
-# conv_stk accumulates, per tap column, KT ceil(Cin / 16) wgmmas of K = 16 (each adds exact 16-bit products with at most
-# one truncation, 2^-23 S: gate 1 of test_gpu_conv_plans.py), then sums the 9 shifted tap partials in fp32 (9 u S) and adds
-# the bias (u S):  E = u (2 KT ceil(Cin / 16) + 10) S,  S = sum |x w| + |bias|.  (A single chain over all 9 KT Cin
-# products would need gate 1's 16 sqrt(K) = 940 u S at KT = 3, Cin = 128; the split keeps it at 58 u S.)
+# Bound: kernel_bounds.conv_stacked_bound, E = u (2 KT ceil(Cin / 16) + 10) S,  S = sum |x w| + |bias|.
 # name: (input [B,T,H,W,Cin], Cout, KT, time offset, pad_t, form); "framed": the SD3 decoder's call - the
 # empty_padded buffer after replicate_border, offset (-tl, 0, 0) - against the conv of the interior with replicate padding
 STK_CASES = {
@@ -389,7 +275,7 @@ def test_conv_stacked16(name, dt):
     f64 = FakeOps(torch.float64)
     r = f64.conv(x, w, bias, out=torch.zeros(y.shape, dtype=torch.float64, device=DEV), **kw)
     S = f64.conv(x.abs(), w.abs(), bias.abs(), out=torch.zeros(y.shape, dtype=torch.float64, device=DEV), **kw)
-    E = U32 * (2 * kt * -(-Ci // 16) + 10) * S
+    E = KB.conv_stacked_bound(S, kt, Ci)
     failed = _gates(f"conv_stacked/{name}/{dt}", y, r, E, dtype)
     assert not failed, "; ".join(failed)
 

@@ -13,7 +13,7 @@ Reference: the operation in fp64 on the same 16-bit inputs.  Gates, one per clas
 """
 import torch
 
-from attention_gates import Gates, gemm_bound, logit_bound, softmax_bound, stats_gate  # noqa: F401  (re-exported)
+from attention_gates import TF32, Gates, gemm_bound, logit_bound, softmax_bound, stats_gate  # noqa: F401  (re-exported)
 from test_gpu_fp32 import _ulp as _ulp_p
 
 U32 = 2.0 ** -24   # unit roundoff of fp32
@@ -32,7 +32,10 @@ MAX_MEAN_ULP = 0.05
 
 
 def _ulp(r, dtype):
-    """Spacing of `dtype` numbers at |r| (r float64), from the exponent bits (test_gpu_fp32._ulp)."""
+    """Spacing of `dtype` numbers at |r| (r float64), from the exponent bits (test_gpu_fp32._ulp); dtype TF32: the
+    store format of fp32 outputs read only by tensor-core products (p = 11, e_min = -126)."""
+    if dtype == TF32:
+        return _ulp_p(r, 11, -126)
     return _ulp_p(r, 11, -14) if dtype == torch.float16 else _ulp_p(r, 8, -126)
 
 
@@ -62,7 +65,8 @@ def _gates(y, r, E, dtype):
 # ------------------------------------------------------------------------------------------------------------ GroupNorm
 # Statistics pass (gn_stats_kernel): each thread sums its 8 channels over P_t = ceil(ppb / lanes) positions in fp32
 # (lanes = 256 / (C / 8) positions per sweep, ppb positions per CTA: pick_grid), then folds min(cpg, 8) channel sums into
-# each of its groups; the square of a 16-bit value is exact in fp32.  Recursive summation of n terms is off by at most
+# each of its groups; the square is exact: a 16-bit value's square fits in fp32, and for fp32 inputs q = fmaf(f, f, q)
+# forms it exactly inside the fma, so in either case each term costs one rounding of the running sum.  Recursive summation of n terms is off by at most
 # n u sum|x_i|, so with eps_sum = (P_t + 7) u the sums are off by eps_sum sum|x| and eps_sum sum x^2.  Each partial is then
 # rounded to the fixed point (1/2 * 2^-20 for the sum, 1/2 * 2^-18 for the squares); a group receives nblocks * lanes *
 # ceil(cpg / 8) partials, N_c per element (fix below).  The block and device sums are exact integers, and the apply

@@ -18,6 +18,16 @@ Gates per call (bounds in tests/kernel_bounds.py and tests/attention_gates.py):
                         the fp64 mean and variance of the handed-in fixed-point sums (the apply kernel alone)
   layernorm, softmax_rows, attn_temporal, conv_stacked   their kernel_bounds references
   copy, replicate_border, pack_taps_hw, blend, pack_weight   bit for bit against fake_ops.FakeOps
+fp32 models (TF32 products) pick their gates by output dtype (the fp32 block of tests/attention_gates.py):
+  conv, GEMM, logits    every tensor-core operand (x, w, sc_x; both operands of a batched GEMM) read with its low 13
+                        mantissa bits truncated, as wgmma .tf32 reads it; bias and residual as they are.  Gate 1 with
+                        1/2 ulp_fp32 and K = 8 per MMA, F (the store stays full fp32), R (closer to the truncating
+                        reading than the round-to-nearest one is, where an operand has low bits)
+  groupnorm, layernorm, softmax_rows   gates 1-3 with TF32 as the store format, and T (low 13 bits zero)
+  attn_temporal         gates 1 and F
+  pack_weight, pack_taps_hw, the channels-first -> channels-last gather   bit for bit against tf32_rn of FakeOps'
+  result; the other movers bit for bit as above.  Each GroupNorm row also records the headroom of the largest 64-bit
+  fixed-point sum of squares below 2^63.
 A conv reference is evaluated on the output frames {0, 1, To/2, To-2, To-1} (all of them when To <= 5; for up_time 2 the
 output frames those conv frames produce) at every H x W position and channel, as a sum over taps of
 [H W, Cin] @ [Cin, Cout] fp64 GEMMs; the batched attention GEMMs are checked in full.
@@ -25,13 +35,16 @@ output frames those conv frames produce) at every H x W position and channel, as
 border nobody filled, fails gate 1.  Any operator-set method outside AUDITED fails the audit, and
 `launch_identity()` proves that every library launch happened inside an audited call.
 """
+import math
 import time
 
 import torch
 
 import kernel_bounds as KB
-from attention_gates import GN_SQ_SCALE, GN_SUM_SCALE, Gates, gemm_bound, logit_bound, stats_compare
+from attention_gates import (GN_SQ_SCALE, GN_SUM_SCALE, TF32, Gates, gemm_bound, kstep, logit_bound, low13,
+                             stats_compare)
 from fake_ops import PAD_REPLICATE, PAD_ZERO, FakeOps
+from test_gpu_fp32 import tf32_rn, tf32_trunc
 
 F64 = torch.float64
 AUDITED = ("empty", "empty_padded", "new_stats", "launch_count", "pack_weight", "conv", "conv_stacked", "groupnorm",
@@ -65,6 +78,30 @@ def same_bits(a, b):
     return a.shape == b.shape and a.dtype == b.dtype and torch.equal(a.view(it), b.view(it))
 
 
+def store_format(dtype):
+    """What the MMA-only producers store: the dtype itself, or TF32 values in fp32 storage."""
+    return TF32 if dtype == torch.float32 else dtype
+
+
+def rounding_copy(x, out):
+    """Whether cvvae_copy5 rounds to TF32: fp32, not the row path, channels-first -> channels-last (the gather of a
+    network input into the channel-padded buffer of the first convolution, its only reader)."""
+    rows = x.stride(3) == 1 and out.stride(3) == 1 and x.shape[4] == out.shape[4] and out.shape[3] > 1
+    return out.dtype == torch.float32 and not rows and x.stride(4) != 1 and out.stride(4) == 1
+
+
+def low_bits_share(t):
+    """Share of the elements of the fp32 tensor t whose low 13 mantissa bits are not all zero (what a TF32 operand read
+    drops), counted in pieces of at most 2^26 elements."""
+    def count(u):
+        if u.numel() <= 1 << 26:
+            return int((low13(u) != 0).sum().item())
+        d = max(range(u.dim()), key=lambda i: u.shape[i])
+        step = max(1, u.shape[d] * (1 << 26) // u.numel())
+        return sum(count(u.narrow(d, a, min(step, u.shape[d] - a))) for a in range(0, u.shape[d], step))
+    return count(t) / max(t.numel(), 1)
+
+
 def _shares(a, b):
     return a is not None and b is not None and a.untyped_storage().data_ptr() == b.untyped_storage().data_ptr()
 
@@ -78,16 +115,18 @@ def _taps(n_out, k, s, off, n_in, mode, device):
 
 def conv_reference(x, w, bias, out_shape, frames, *, kernel=(1, 1, 1), stride=(1, 1, 1), offset=(0, 0, 0),
                    pad_t=PAD_ZERO, pad_hw=PAD_ZERO, up_time=1, alpha=1.0, residual=None, sc_x=None, sc_w=None,
-                   cout=None):
+                   cout=None, operand=None):
     """FakeOps.conv in fp64 on the conv frames `frames`: (output frame indices, r, S) with r, S [B, frames, Ho, Wo, C]
-    and S the same sum on absolute values.  Out-of-range taps are clamped (replicate) or contribute zero."""
+    and S the same sum on absolute values.  Out-of-range taps are clamped (replicate) or contribute zero.  operand: how
+    the tensor cores read x, w and sc_x (tf32_trunc for fp32 storage), applied before the products."""
+    op = operand or (lambda t: t)
     kt, kh, kw = kernel
     st, sh, sw = stride
     B, T, H, W, Ci = x.shape
     Co = cout if cout is not None else w.shape[1]
     Ho, Wo = out_shape[2], out_shape[3]
     dev = x.device
-    wt = w[:, :Co, :Ci].double()
+    wt = op(w[:, :Co, :Ci]).double()
     wa = wt.abs()
     hi, hv = _taps(Ho, kh, sh, offset[1], H, pad_hw, dev)
     wi, wv = _taps(Wo, kw, sw, offset[2], W, pad_hw, dev)
@@ -108,7 +147,7 @@ def conv_reference(x, w, bias, out_shape, frames, *, kernel=(1, 1, 1), stride=(1
                     xab = xa.index_select(2, wi[b])
                     if wv is not None:
                         xab = torch.where(wv[b].view(1, 1, -1, 1), xab, torch.zeros((), dtype=xab.dtype, device=dev))
-                    X = xab.reshape(-1, Ci).double()
+                    X = op(xab.reshape(-1, Ci)).double()
                     tap = (j * kh + a) * kw + b
                     r[:, fi] += (X @ wt[tap].T).view(B, Ho, Wo, Co)
                     S[:, fi] += (X.abs() @ wa[tap].T).view(B, Ho, Wo, Co)
@@ -132,9 +171,9 @@ def conv_reference(x, w, bias, out_shape, frames, *, kernel=(1, 1, 1), stride=(1
     else:
         of = list(frames)
     if sc_w is not None:
-        xs = sc_x[:, of].double()
-        r += xs @ sc_w.double().T
-        S += xs.abs() @ sc_w.double().abs().T
+        xs = op(sc_x[:, of]).double()
+        r += xs @ op(sc_w).double().T
+        S += xs.abs() @ op(sc_w).double().abs().T
     if residual is not None:
         rr = residual[:, of].double()
         r += rr
@@ -203,7 +242,8 @@ class AuditOps:
 
     def _gate_fields(self, gates):
         rec, failed = gates.result()
-        keep = ("worst_bound_ratio", "correctly_rounded_share", "mean_signed_ulp", "numel")
+        keep = ("worst_bound_ratio", "correctly_rounded_share", "mean_signed_ulp", "numel", "tf32_valued_share",
+                "rms_error_ratio", "rn_separation", "error_over_separation", "low_bits_set")
         return {k: rec[k] for k in keep if k in rec}, failed
 
     # ---------------------------------------------------------------- memory (NaN-filled)
@@ -236,7 +276,8 @@ class AuditOps:
     def pack_weight(self, w):
         t0 = time.perf_counter()
         y, n = self._run(self.inner.pack_weight, w)
-        ok = same_bits(y, self._fake.pack_weight(w))
+        ref = self._fake.pack_weight(w)
+        ok = same_bits(y, tf32_rn(ref) if w.dtype == torch.float32 else ref)
         self._row("pack_weight", n, self._layer(w), [] if ok else ["bits differ from FakeOps.pack_weight"], t0,
                   shape_in=list(w.shape))
         return y
@@ -247,9 +288,11 @@ class AuditOps:
         y, n = self._run(self.inner.copy, x, out)
         ref = torch.full(out.shape, float("nan"), dtype=out.dtype, device=out.device)
         self._fake.copy(xs, ref)
-        ok = same_bits(out, ref)
+        rounded = rounding_copy(x, out)
+        ok = same_bits(out, tf32_rn(ref) if rounded else ref)
         self._row("copy", n, self._layer(), [] if ok else ["bits differ from FakeOps.copy"], t0,
-                  shape_in=list(x.shape), shape_out=list(out.shape), view=view_kind(out), view_in=view_kind(x))
+                  shape_in=list(x.shape), shape_out=list(out.shape), view=view_kind(out), view_in=view_kind(x),
+                  tf32_rounded=rounded)
         return y
 
     def replicate_border(self, xpad):
@@ -266,7 +309,7 @@ class AuditOps:
         y, n = self._run(self.inner.pack_taps_hw, x, out, kh, kw, offset=offset, pad_hw=pad_hw)
         ref = torch.full(out.shape, float("nan"), dtype=out.dtype, device=out.device)
         self._fake.pack_taps_hw(x, ref, kh, kw, offset=offset, pad_hw=pad_hw)
-        ok = same_bits(out, ref)
+        ok = same_bits(out, tf32_rn(ref) if out.dtype == torch.float32 else ref)
         self._row("pack_taps_hw", n, self._layer(), [] if ok else ["bits differ from FakeOps.pack_taps_hw"], t0,
                   shape_in=list(x.shape), shape_out=list(out.shape), view_in=view_kind(x))
         return y
@@ -301,8 +344,27 @@ class AuditOps:
                   "kernel": list(kernel), "stride": list(kw.get("stride", (1, 1, 1))), "up_time": kw.get("up_time", 1),
                   "shortcut": kw.get("sc_w") is not None, "residual": kw.get("residual") is not None,
                   "out_f32": bool(kw.get("out_f32")), "batched": bool(batched)}
+        plan_fn = getattr(self.inner, "conv_tc_plan", None)
+        plan = None
+        if plan_fn is not None:
+            plan = plan_fn(x, w, bias, epilogue=True, **{k: v for k, v in kw.items() if k in _DESC_KW})
+            fields["plan"] = {k: plan[k] for k in PLAN_FIELDS}
+        f32 = x.dtype == torch.float32     # an fp32 model (the logits of a 16-bit one are fp32 too)
+        tc = plan is None or bool(plan["eligible"])     # the operator sets without a plan query stand for conv_tc
+        # fp32: the tensor cores read x, w and sc_x truncated to TF32, K = 8 products per MMA; the CUDA-core conv reads
+        # them whole, one fma rounding per product (the linear bound with one product per step)
+        ks = (8 if tc else 1) if f32 else kstep(x.dtype)
+        op = tf32_trunc if f32 and tc else None
+        rn = False       # gate R: also the reference with operands rounded to nearest, where an operand has low bits
+        if f32:
+            fields["x_low_bits_share"] = low_bits_share(x)
+            if batched:
+                fields["w_low_bits_share"] = low_bits_share(w)
+            if kw.get("sc_w") is not None:
+                fields["sc_x_low_bits_share"] = low_bits_share(ref_kw["sc_x"])
+            rn = tc and max(v for k, v in fields.items() if k.endswith("low_bits_share")) > 0
         if kw.get("out_f32"):
-            gates = Gates(None)
+            gates = Gates(torch.float32 if f32 else None)
         else:
             gates = Gates(dtype, K=K)
         if batched:
@@ -310,24 +372,35 @@ class AuditOps:
             a32 = float(torch.tensor(alpha, dtype=torch.float32))
             Co = kw.get("cout") or w.shape[1]
             for bi in range(out.shape[0]):
-                X = x[0 if kw.get("x_shared") else bi].reshape(-1, x.shape[4]).double()
-                Wm = w[bi if kw.get("w_per_batch") else 0][:Co, :x.shape[4]].double()
+                X = x[0 if kw.get("x_shared") else bi].reshape(-1, x.shape[4])
+                Wm = w[bi if kw.get("w_per_batch") else 0][:Co, :x.shape[4]]
+                r_rn = (tf32_rn(X).double() @ tf32_rn(Wm).double().T) if rn else None
+                X, Wm = (op(X), op(Wm)) if op else (X, Wm)
+                X, Wm = X.double(), Wm.double()
                 yb = out[bi].reshape(X.shape[0], Co)
                 if kw.get("out_f32"):
                     r = a32 * (X @ Wm.T)
-                    gates.add(yb, r, logit_bound(x.shape[4], a32, X.abs() @ Wm.abs().T, r))
+                    gates.add(yb, r, logit_bound(x.shape[4], a32, X.abs() @ Wm.abs().T, r, ks),
+                              r_rn=a32 * r_rn if rn else None)
                     continue
                 r, S = alpha * (X @ Wm.T), abs(alpha) * (X.abs() @ Wm.abs().T)
                 if bias is not None:
                     bb = bias.double().view(-1, 1) if kw.get("bias_along_m") else bias.double().view(1, -1)
                     r, S = r + bb, S + bb.abs()
-                gates.add(yb, r, gemm_bound(K, S))
+                    r_rn = alpha * r_rn + bb if rn else None
+                elif rn:
+                    r_rn = alpha * r_rn
+                gates.add(yb, r, gemm_bound(K, S, ks), r_rn=r_rn)
                 del X, Wm, r, S
         else:
             To = (out.shape[1] + 1) // 2 if kw.get("up_time", 1) == 2 else out.shape[1]
-            of, r, S = conv_reference(x, w, bias, tuple(out.shape), sample_frames(To), **ref_kw)
+            of, r, S = conv_reference(x, w, bias, tuple(out.shape), sample_frames(To), operand=op, **ref_kw)
+            r_rn = None
+            if rn:
+                r_rn = conv_reference(x, w, bias, tuple(out.shape), sample_frames(To), operand=tf32_rn, **ref_kw)[1]
             fields["frames_checked"] = of
-            gates.add(out[:, of], r, gemm_bound(K, S))
+            gates.add(out[:, of], r, gemm_bound(K, S, ks), r_rn=r_rn)
+            del r_rn
             del r, S
         vals, failed = self._gate_fields(gates)
         fields.update(vals)
@@ -337,10 +410,6 @@ class AuditOps:
             err, f_st = stats_compare(group_sums(out, groups), st - before)
             fields["stats_max_abs_err"] = err
             failed = failed + f_st
-        plan_fn = getattr(self.inner, "conv_tc_plan", None)
-        if plan_fn is not None:
-            p = plan_fn(x, w, bias, epilogue=True, **{k: v for k, v in kw.items() if k in _DESC_KW})
-            fields["plan"] = {k: p[k] for k in PLAN_FIELDS}
         self._row("conv", n, self._layer(w, x, bias), failed, t0, **fields)
         return y
 
@@ -380,7 +449,8 @@ class AuditOps:
     def _groupnorm_gates(self, x, y, gamma, beta, groups, eps, per_frame, silu, stats):
         B, T, H, W, Cc = x.shape
         cpg = Cc // groups
-        gates = Gates(y.dtype)
+        gates = Gates(store_format(y.dtype))
+        sq_max = 0.0        # the largest fixed-point sum of squares of a statistics unit (a sample, or a frame)
         fields = {"shape_in": list(x.shape), "view_in": view_kind(x), "view": view_kind(y), "per_frame": per_frame,
                   "silu": silu, "handed_in_stats": stats is not None}
         if per_frame:
@@ -388,6 +458,8 @@ class AuditOps:
             for t in range(T):
                 r, E, _ = KB.gn_reference(x[:, t:t + 1], gamma, beta, groups, eps, True, silu, eps_sum, fix)
                 gates.add(y[:, t:t + 1], r, E)
+                v = x[:, t].double().reshape(B, -1, groups, cpg)
+                sq_max = max(sq_max, (v * v).sum(dim=(1, 3)).max().item())
         else:
             cnt = T * H * W * cpg
             if stats is None:
@@ -401,6 +473,7 @@ class AuditOps:
                     sa += v.abs().sum(dim=(1, 3), keepdim=True)
                 mean, sqmean, absmean = s1 / cnt, s2 / cnt, sa / cnt
                 var = (sqmean - mean * mean).clamp_min(0)
+                sq_max = s2.max().item()
             else:
                 st = stats.double()
                 mean = (st[:, :, 0] / GN_SUM_SCALE / cnt).view(B, 1, groups, 1)
@@ -408,6 +481,7 @@ class AuditOps:
                 var = var.clamp_min(0)
                 absmean = sqmean = None
                 eps_sum, fix = None, cnt
+                sq_max = st[:, :, 1].max().item() / GN_SQ_SCALE
             kmax = 0.0
             for t in range(T):
                 v = x[:, t].double().reshape(B, -1, groups, cpg)
@@ -416,6 +490,8 @@ class AuditOps:
                 gates.add(y[:, t].reshape(r.shape), r, E)
                 del v, r, E
             fields["max_mean_over_std"] = kmax
+        # DESIGN section 6: the sums are 64-bit fixed point (sum of squares * 2^18); bits left below 2^63 (recorded only)
+        fields["sq_headroom_bits"] = math.log2(2.0 ** 63 / max(sq_max * GN_SQ_SCALE, 1.0))
         vals, failed = self._gate_fields(gates)
         return vals, failed, fields
 
@@ -423,7 +499,7 @@ class AuditOps:
         t0 = time.perf_counter()
         y, n = self._run(self.inner.layernorm, x, gamma, beta, eps)
         r, E, k = KB.layernorm_reference(x, gamma, beta, eps)
-        vals, failed = self._gate_fields(Gates(y.dtype).add(y, r, E))
+        vals, failed = self._gate_fields(Gates(store_format(y.dtype)).add(y, r, E))
         self._row("layernorm", n, self._layer(gamma), failed, t0, shape_in=list(x.shape), max_mean_over_std=k, **vals)
         return y
 
@@ -431,7 +507,7 @@ class AuditOps:
         t0 = time.perf_counter()
         y, n = self._run(self.inner.softmax_rows, s, cols, out)
         r, E = KB.softmax_reference(s, cols)
-        vals, failed = self._gate_fields(Gates(out.dtype).add(out[:, :cols], r, E))
+        vals, failed = self._gate_fields(Gates(store_format(out.dtype)).add(out[:, :cols], r, E))
         self._row("softmax_rows", n, self._layer(), failed, t0, shape_in=list(s.shape), cols=cols, **vals)
         return y
 
@@ -439,7 +515,8 @@ class AuditOps:
         t0 = time.perf_counter()
         y, n = self._run(self.inner.attn_temporal, q, k, v)
         r, E, _ = KB.attn_temporal_reference(q, k, v)
-        vals, failed = self._gate_fields(Gates(y.dtype).add(y, r, E))
+        # fp32: CUDA cores, no operand truncation; the store is full fp32 (gates 1 and F)
+        vals, failed = self._gate_fields(Gates(y.dtype, rms=False).add(y, r, E))
         self._row("attn_temporal", n, self._layer(), failed, t0, shape_in=list(q.shape), **vals)
         return y
 

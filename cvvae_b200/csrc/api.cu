@@ -1,6 +1,7 @@
-// Library-wide state of libcvvae_b200 (error string, launch counter, driver entry point) and the
-// shared-memory matrix descriptor probe used by the GPU test-suite.
+// Library-wide state of libcvvae_b200 (error string, launch counter, driver entry point), the tensor-map builders every
+// TMA kernel uses, and the shared-memory matrix descriptor probe used by the GPU test-suite.
 #include <stdarg.h>
+#include <stdlib.h>
 #include <string.h>
 
 #include "common.cuh"
@@ -30,6 +31,101 @@ PFN_encodeTiled get_encode_tiled() {
       fn = reinterpret_cast<PFN_encodeTiled>(p);
   }
   return fn;
+}
+
+// cuTensorMapEncodeTiled is a pure function of its arguments and costs 1-2 us on the host; a network pass issues the same
+// few hundred (pointer, shape) combinations call after call (the activation buffers come back from the caching allocator at
+// the same addresses), so the encoded maps are memoised per thread, keyed by the full argument list (SURVEY 8b: "optional
+// descriptor cache keyed by (ptr, shape)").
+struct TmapKey {
+  const void* ptr;
+  uint32_t rank, swizzle, esz;
+  cuuint64_t dims[5], strides[4];
+  cuuint32_t box[5], estr[5];
+  bool operator==(const TmapKey& o) const { return memcmp(this, &o, sizeof(TmapKey)) == 0; }
+};
+struct TmapSlot {
+  TmapKey key;
+  CUtensorMap map;
+  bool valid;
+};
+static constexpr int kTmapSlots = 1024;
+
+bool encode_map(CUtensorMap* m, const void* ptr, int rank, const cuuint64_t* dims, const cuuint64_t* strides_b,
+                const cuuint32_t* box, const cuuint32_t* estr, int esz, CUtensorMapSwizzle swizzle) {
+  static thread_local TmapSlot* cache = nullptr;
+  if (!cache) cache = static_cast<TmapSlot*>(calloc(kTmapSlots, sizeof(TmapSlot)));
+  TmapKey key;
+  memset(&key, 0, sizeof(key));
+  key.ptr = ptr;
+  key.rank = static_cast<uint32_t>(rank);
+  key.swizzle = static_cast<uint32_t>(swizzle);
+  key.esz = static_cast<uint32_t>(esz);
+  for (int i = 0; i < rank; ++i) {
+    key.dims[i] = dims[i];
+    key.box[i] = box[i];
+    key.estr[i] = estr[i];
+    if (i + 1 < rank) key.strides[i] = strides_b[i];
+  }
+  uint64_t h = 1469598103934665603ull;  // FNV-1a over the key bytes
+  const unsigned char* kb = reinterpret_cast<const unsigned char*>(&key);
+  for (size_t i = 0; i < sizeof(key); ++i) h = (h ^ kb[i]) * 1099511628211ull;
+  TmapSlot* slot = cache ? &cache[h % kTmapSlots] : nullptr;
+  if (slot && slot->valid && slot->key == key) {
+    *m = slot->map;
+    return true;
+  }
+  PFN_encodeTiled enc = get_encode_tiled();
+  if (!enc) {
+    set_error("cuTensorMapEncodeTiled entry point not available");
+    return false;
+  }
+  CUresult r = enc(m, esz == 4 ? CU_TENSOR_MAP_DATA_TYPE_UINT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16, rank, const_cast<void*>(ptr), dims, strides_b, box, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeTiled failed (CUresult %d): rank %d dims [%llu %llu %llu %llu %llu] box [%u %u %u %u %u]",
+              (int)r, rank, (unsigned long long)dims[0], (unsigned long long)(rank > 1 ? dims[1] : 0),
+              (unsigned long long)(rank > 2 ? dims[2] : 0), (unsigned long long)(rank > 3 ? dims[3] : 0),
+              (unsigned long long)(rank > 4 ? dims[4] : 0), box[0], rank > 1 ? box[1] : 0, rank > 2 ? box[2] : 0,
+              rank > 3 ? box[3] : 0, rank > 4 ? box[4] : 0);
+    return false;
+  }
+  if (slot) {
+    slot->key = key;
+    slot->map = *m;
+    slot->valid = true;
+  }
+  return true;
+}
+
+bool tma_view(const cvvae_tensor5& t, int esz, cuuint64_t* dims, cuuint64_t* strides) {
+  if (t.s_c != 1 || reinterpret_cast<uintptr_t>(t.ptr) % 16) return false;
+  const long long s[4] = {t.s_w, t.s_h, t.s_t, t.s_b};
+  const int n[5] = {t.C, t.W, t.H, t.T, t.B};
+  for (int i = 0; i < 4; ++i)
+    if (n[i + 1] > 1 && (s[i] <= 0 || (s[i] * esz) % 16)) return false;
+  for (int i = 0; i < 5 && dims; ++i) dims[i] = static_cast<cuuint64_t>(n[i]);
+  for (int i = 0; i < 4 && strides; ++i)
+    strides[i] = n[i + 1] == 1 ? (static_cast<cuuint64_t>(t.C) * esz + 15) & ~cuuint64_t(15) : static_cast<cuuint64_t>(s[i]) * esz;
+  return true;
+}
+
+bool act_map(CUtensorMap* m, const cvvae_tensor5& t, int esz, const cuuint32_t box[5], const cuuint32_t estr[5]) {
+  cuuint64_t dims[5], strides[4];
+  if (!tma_view(t, esz, dims, strides)) {
+    set_error("tensor map: not a 16-byte aligned channels-last view");
+    return false;
+  }
+  return encode_map(m, t.ptr, 5, dims, strides, box, estr, esz);
+}
+
+bool weight_map(CUtensorMap* m, const void* w, long long K, long long rows, long long mats, long long ld, int esz,
+                uint32_t box_k, uint32_t box_rows) {
+  const cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)rows, (cuuint64_t)mats};
+  const cuuint64_t strides[2] = {(cuuint64_t)(ld * esz), (cuuint64_t)(ld * rows * esz)};
+  const cuuint32_t box[3] = {box_k, box_rows, 1}, estr[3] = {1, 1, 1};
+  return encode_map(m, w, 3, dims, strides, box, estr, esz);
 }
 
 // One warpgroup: TMA a [rows_total][64] 16-bit matrix and a [N][64] matrix into SWIZZLE_128B shared memory, run a
@@ -99,29 +195,11 @@ extern "C" int cvvae_probe_umma_shift(const void* a_rows, const void* b_rows, fl
   CVVAE_CHECK_ARG(a_rows && b_rows && out && (n == 64 || n == 128 || n == 256) && row_shift >= 0 && row_shift <= 64 &&
                       sbo_rows >= 8 && sbo_rows <= 16,
                   "cvvae_probe_umma_shift: bad argument");
-  PFN_encodeTiled enc = get_encode_tiled();
-  CVVAE_CHECK_ARG(enc, "cuTensorMapEncodeTiled entry point not available");
   const int rows_total = 320;   // 15 groups x 16 rows + 8 + shift 64 <= 320
   CUtensorMap tmA, tmB;
-  cuuint32_t estr[3] = {1, 1, 1};
-  {
-    cuuint64_t dims[3] = {64, (cuuint64_t)rows_total, 1};
-    cuuint64_t strides[2] = {128, 128ull * rows_total};
-    cuuint32_t box[3] = {64, (cuuint32_t)(rows_total / 2), 1};
-    CUresult r = enc(&tmA, CU_TENSOR_MAP_DATA_TYPE_UINT16, 3, const_cast<void*>(a_rows), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    CVVAE_CHECK_ARG(r == CUDA_SUCCESS, "probe: tensor map A failed (%d)", (int)r);
-  }
-  {
-    cuuint64_t dims[3] = {64, (cuuint64_t)n, 1};
-    cuuint64_t strides[2] = {128, 128ull * n};
-    cuuint32_t box[3] = {64, (cuuint32_t)n, 1};
-    CUresult r = enc(&tmB, CU_TENSOR_MAP_DATA_TYPE_UINT16, 3, const_cast<void*>(b_rows), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    CVVAE_CHECK_ARG(r == CUDA_SUCCESS, "probe: tensor map B failed (%d)", (int)r);
-  }
+  if (!weight_map(&tmA, a_rows, 64, rows_total, 1, 64, 2, 64, rows_total / 2) ||
+      !weight_map(&tmB, b_rows, 64, n, 1, 64, 2, 64, n))
+    return CVVAE_E_ARG;
   const size_t smem = 1024 + 49152 + 32768 + 64;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (n == 64) {

@@ -52,6 +52,22 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
                                     CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 PFN_encodeTiled get_encode_tiled();
 
+// ---- tensor maps (api.cu): SWIZZLE_128B by default, 256-B L2 promotion, memoised per thread.  Each returns false with
+// the error set when the driver refuses the map.
+bool encode_map(CUtensorMap* m, const void* ptr, int rank, const cuuint64_t* dims, const cuuint64_t* strides_b,
+                const cuuint32_t* box, const cuuint32_t* estr, int esz, CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B);
+// Whether TMA can address t as a 5-D channels-last view of esz-byte elements: channel stride 1, a 16-byte aligned
+// pointer, and a positive 16-byte multiple of a stride on every axis of extent > 1.  An axis of extent 1 is never read
+// along, so it may carry any stride and gets a valid one.  When dims / strides are given, they receive the map's
+// extents {C, W, H, T, B} and byte strides {W, H, T, B}.
+bool tma_view(const cvvae_tensor5& t, int esz, cuuint64_t* dims = nullptr, cuuint64_t* strides = nullptr);
+// A channels-last activation view (which must pass tma_view) as a 5-D map.
+bool act_map(CUtensorMap* m, const cvvae_tensor5& t, int esz, const cuuint32_t box[5], const cuuint32_t estr[5]);
+// A packed [mats][rows][ld] matrix stack whose first K elements per row are data, as a 3-D map with box
+// {box_k, box_rows, 1}.
+bool weight_map(CUtensorMap* m, const void* w, long long K, long long rows, long long mats, long long ld, int esz,
+                uint32_t box_k, uint32_t box_rows);
+
 // fp32 -> nearest TF32 value (ties to even), kept in fp32 storage with the low 13 mantissa bits zero.  Written out in
 // integer arithmetic so that it is the same function everywhere (kernels and the test-suite's reference).
 __device__ __forceinline__ float tf32_rn(float v) {

@@ -78,28 +78,27 @@ __global__ void __launch_bounds__(kStkThreads, 1)
 
   if (threadIdx.x < 128) {
     ptx::setmaxnreg_dec<40>();
-    int slot = 0;
-    uint32_t phase = 0;
+    ptx::Ring r;
     if (warp == 0) {
       for_each_step([&](int kt, int ti, int cb) {
-        ptx::mbar_wait(&emptyA[slot], phase ^ 1);
+        ptx::mbar_wait(&emptyA[r.slot], r.phase ^ 1);
         if (ptx::elect_one()) {
-          ptx::mbar_expect_tx(&fullA[slot], kSlabBytes);
+          ptx::mbar_expect_tx(&fullA[r.slot], kSlabBytes);
           // slab position (0,0) is the input position of output (h0,w0) at tap (0,0)
-          ptx::tma_load_5d(sA + slot * kSlabBytes, &tmA, &fullA[slot], cb * 64, w0 + p.off_w, h0 + p.off_h, ti, b);
+          ptx::tma_load_5d(sA + r.slot * kSlabBytes, &tmA, &fullA[r.slot], cb * 64, w0 + p.off_w, h0 + p.off_h, ti, b);
         }
         __syncwarp();
-        if (++slot == kNA) { slot = 0; phase ^= 1; }
+        r.advance(kNA);
       });
     } else if (warp == 1) {
       for_each_step([&](int kt, int ti, int cb) {
-        ptx::mbar_wait(&emptyB[slot], phase ^ 1);
+        ptx::mbar_wait(&emptyB[r.slot], r.phase ^ 1);
         if (ptx::elect_one()) {
-          ptx::mbar_expect_tx(&fullB[slot], kBBytes);
-          ptx::tma_load_3d(sB + slot * kBBytes, &tmB, &fullB[slot], cb * 64, 0, kt);
+          ptx::mbar_expect_tx(&fullB[r.slot], kBBytes);
+          ptx::tma_load_3d(sB + r.slot * kBBytes, &tmB, &fullB[r.slot], cb * 64, 0, kt);
         }
         __syncwarp();
-        if (++slot == kNB) { slot = 0; phase ^= 1; }
+        r.advance(kNB);
       });
     }
     return;
@@ -111,15 +110,16 @@ __global__ void __launch_bounds__(kStkThreads, 1)
   const bool wg_leader = (threadIdx.x & 127) == 0;
   float acc[kChunks][kNstk / 2];
   {
-    int slotA = 0, slotB = 0, pendA = -1, pendB = -1;
-    uint32_t phaseA = 0, phaseB = 0, accumulate = 0;
+    ptx::Ring ra, rb;
+    int pendA = -1, pendB = -1;
+    uint32_t accumulate = 0;
     for_each_step([&](int kt, int ti, int cb) {
-      ptx::mbar_wait(&fullA[slotA], phaseA);
-      ptx::mbar_wait(&fullB[slotB], phaseB);
+      ptx::mbar_wait(&fullA[ra.slot], ra.phase);
+      ptx::mbar_wait(&fullB[rb.slot], rb.phase);
       const int ch_left = p.Cin - cb * 64;
       const int ksteps = ch_left >= 64 ? 4 : (ch_left + 15) >> 4;
-      const uint32_t a0 = ptx::smem_u32(sA + slotA * kSlabBytes) + static_cast<uint32_t>(half * kChunks * 64) * 128u;
-      const uint32_t b0 = ptx::smem_u32(sB + slotB * kBBytes);
+      const uint32_t a0 = ptx::smem_u32(sA + ra.slot * kSlabBytes) + static_cast<uint32_t>(half * kChunks * 64) * 128u;
+      const uint32_t b0 = ptx::smem_u32(sB + rb.slot * kBBytes);
       ptx::wgmma_fence();
 #pragma unroll
       for (int c = 0; c < kChunks; ++c)
@@ -135,10 +135,10 @@ __global__ void __launch_bounds__(kStkThreads, 1)
         ptx::mbar_arrive(&emptyB[pendB]);
         ptx::mbar_arrive(&emptyA[pendA]);
       }
-      pendA = slotA;
-      pendB = slotB;
-      if (++slotA == kNA) { slotA = 0; phaseA ^= 1; }
-      if (++slotB == kNB) { slotB = 0; phaseB ^= 1; }
+      pendA = ra.slot;
+      pendB = rb.slot;
+      ra.advance(kNA);
+      rb.advance(kNB);
     });
     ptx::wgmma_wait<0>();
 #pragma unroll
@@ -207,16 +207,13 @@ extern "C" int cvvae_conv3d_stacked(const cvvae_conv_desc* d, void* stream_) {
   CVVAE_CHECK_ARG(d->Cout >= 1 && d->Cout <= 4 && y.C == d->Cout, "cvvae_conv3d_stacked: Cout %d not in 1..4", d->Cout);
   CVVAE_CHECK_ARG(!d->residual && !d->gn_stats && !(d->flags & (CVVAE_CONV_OUT_F32 | CVVAE_CONV_BIAS_ALONG_M)),
                   "cvvae_conv3d_stacked: residual / statistics / fp32 output are not supported");
-  CVVAE_CHECK_ARG(x.s_c == 1 && !(x.s_w % 8) && !(x.s_h % 8) && !(x.s_t % 8) && !(x.s_b % 8) &&
-                      reinterpret_cast<uintptr_t>(x.ptr) % 16 == 0 && reinterpret_cast<uintptr_t>(d->w) % 16 == 0 && x.C % 8 == 0,
+  CVVAE_CHECK_ARG(tma_view(x, 2) && reinterpret_cast<uintptr_t>(d->w) % 16 == 0 && x.C % 8 == 0,
                   "cvvae_conv3d_stacked: input must be a 16-byte aligned channels-last view");
   if (d->pad_hw != CVVAE_PAD_ZERO) {
     const int hi_h = (y.H - 1) + 2 + d->off_h, hi_w = (y.W - 1) + 2 + d->off_w;
     CVVAE_CHECK_ARG(d->off_h >= 0 && d->off_w >= 0 && hi_h < x.H && hi_w < x.W,
                     "cvvae_conv3d_stacked: replicate H/W padding needs a pre-padded (framed) input");
   }
-  PFN_encodeTiled enc = get_encode_tiled();
-  CVVAE_CHECK_ARG(enc, "cuTensorMapEncodeTiled entry point not available");
   ConvStkParams p{};
   p.B = x.B; p.T_in = x.T; p.T_out = y.T; p.H_out = y.H; p.W_out = y.W; p.Cin = x.C; p.Cout = d->Cout;
   p.KT = d->KT; p.off_t = d->off_t; p.off_h = d->off_h; p.off_w = d->off_w; p.pad_t = d->pad_t;
@@ -227,25 +224,8 @@ extern "C" int cvvae_conv3d_stacked(const cvvae_conv_desc* d, void* stream_) {
   p.cblocks = (p.Cin + 63) / 64;
   p.xstride = (9 * p.Cout) | 1;  // odd stride: conflict-free for consecutive positions
   CUtensorMap tmA, tmB;
-  {
-    cuuint64_t dims[5] = {(cuuint64_t)x.C, (cuuint64_t)x.W, (cuuint64_t)x.H, (cuuint64_t)x.T, (cuuint64_t)x.B};
-    cuuint64_t strides[4] = {(cuuint64_t)x.s_w * 2, (cuuint64_t)x.s_h * 2, (cuuint64_t)x.s_t * 2, (cuuint64_t)x.s_b * 2};
-    for (int i = 0; i < 4; ++i)
-      if (dims[i + 1] == 1 && (strides[i] == 0 || strides[i] % 16)) strides[i] = (cuuint64_t)x.C * 2;
-    cuuint32_t box[5] = {64, kSlabW, kSlabH, 1, 1}, estr[5] = {1, 1, 1, 1, 1};
-    CUresult r = enc(&tmA, CU_TENSOR_MAP_DATA_TYPE_UINT16, 5, x.ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    CVVAE_CHECK_ARG(r == CUDA_SUCCESS, "cvvae_conv3d_stacked: tensor map A failed (%d)", (int)r);
-  }
-  {
-    cuuint64_t dims[3] = {(cuuint64_t)p.Cin, (cuuint64_t)kNstk, (cuuint64_t)p.KT};
-    cuuint64_t strides[2] = {(cuuint64_t)p.Cin * 2, (cuuint64_t)p.Cin * kNstk * 2};
-    cuuint32_t box[3] = {64, kNstk, 1}, estr[3] = {1, 1, 1};
-    CUresult r = enc(&tmB, CU_TENSOR_MAP_DATA_TYPE_UINT16, 3, const_cast<void*>(d->w), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    CVVAE_CHECK_ARG(r == CUDA_SUCCESS, "cvvae_conv3d_stacked: tensor map B failed (%d)", (int)r);
-  }
+  const cuuint32_t box[5] = {64, kSlabW, kSlabH, 1, 1}, estr[5] = {1, 1, 1, 1, 1};
+  if (!act_map(&tmA, x, 2, box, estr) || !weight_map(&tmB, d->w, p.Cin, kNstk, p.KT, p.Cin, 2, 64, kNstk)) return CVVAE_E_ARG;
   const long long grid = 1ll * p.T_out * p.tiles_w * p.tiles_h * p.B;
   CVVAE_CHECK_ARG(grid > 0 && grid < (1ll << 31), "cvvae_conv3d_stacked: grid out of range");
   const size_t smem = 1024 + kNA * kSlabBytes + kNB * kBBytes + 256;

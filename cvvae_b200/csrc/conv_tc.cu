@@ -690,76 +690,9 @@ __global__ void __launch_bounds__(kThreads, 1)
 }
 
 // ---------------------------------------------------------------------------------------- host side
-// cuTensorMapEncodeTiled is a pure function of its arguments and costs 1-2 us on the host; a network pass issues the same
-// few hundred (pointer, shape) combinations call after call (the activation buffers come back from the caching allocator at
-// the same addresses), so the encoded maps are memoised per thread, keyed by the full argument list (SURVEY 8b: "optional
-// descriptor cache keyed by (ptr, shape)").
-struct TmapKey {
-  const void* ptr;
-  uint32_t rank, swizzle, esz;
-  cuuint64_t dims[5], strides[4];
-  cuuint32_t box[5], estr[5];
-  bool operator==(const TmapKey& o) const { return memcmp(this, &o, sizeof(TmapKey)) == 0; }
-};
-struct TmapSlot {
-  TmapKey key;
-  CUtensorMap map;
-  bool valid;
-};
-static constexpr int kTmapSlots = 1024;
-
 // Element size of an activation dtype in bytes, and channels per 128-byte operand row.
 static int elem_bytes(int dtype) { return dtype == CVVAE_F32 ? 4 : 2; }
 static int chan_block(int dtype) { return 128 / elem_bytes(dtype); }
-
-static bool encode_map(CUtensorMap* m, const void* ptr, int rank, const cuuint64_t* dims, const cuuint64_t* strides_b,
-                       const cuuint32_t* box, const cuuint32_t* estr, int esz,
-                       CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
-  static thread_local TmapSlot* cache = nullptr;
-  if (!cache) cache = static_cast<TmapSlot*>(calloc(kTmapSlots, sizeof(TmapSlot)));
-  TmapKey key;
-  memset(&key, 0, sizeof(key));
-  key.ptr = ptr;
-  key.rank = static_cast<uint32_t>(rank);
-  key.swizzle = static_cast<uint32_t>(swizzle);
-  key.esz = static_cast<uint32_t>(esz);
-  for (int i = 0; i < rank; ++i) {
-    key.dims[i] = dims[i];
-    key.box[i] = box[i];
-    key.estr[i] = estr[i];
-    if (i + 1 < rank) key.strides[i] = strides_b[i];
-  }
-  uint64_t h = 1469598103934665603ull;  // FNV-1a over the key bytes
-  const unsigned char* kb = reinterpret_cast<const unsigned char*>(&key);
-  for (size_t i = 0; i < sizeof(key); ++i) h = (h ^ kb[i]) * 1099511628211ull;
-  TmapSlot* slot = cache ? &cache[h % kTmapSlots] : nullptr;
-  if (slot && slot->valid && slot->key == key) {
-    *m = slot->map;
-    return true;
-  }
-  PFN_encodeTiled enc = get_encode_tiled();
-  if (!enc) {
-    set_error("cuTensorMapEncodeTiled entry point not available");
-    return false;
-  }
-  CUresult r = enc(m, esz == 4 ? CU_TENSOR_MAP_DATA_TYPE_UINT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16, rank, const_cast<void*>(ptr), dims, strides_b, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled failed (CUresult %d): rank %d dims [%llu %llu %llu %llu %llu] box [%u %u %u %u %u]",
-              (int)r, rank, (unsigned long long)dims[0], (unsigned long long)(rank > 1 ? dims[1] : 0),
-              (unsigned long long)(rank > 2 ? dims[2] : 0), (unsigned long long)(rank > 3 ? dims[3] : 0),
-              (unsigned long long)(rank > 4 ? dims[4] : 0), box[0], rank > 1 ? box[1] : 0, rank > 2 ? box[2] : 0,
-              rank > 3 ? box[3] : 0, rank > 4 ? box[4] : 0);
-    return false;
-  }
-  if (slot) {
-    slot->key = key;
-    slot->map = *m;
-    slot->valid = true;
-  }
-  return true;
-}
 
 bool conv_tc_eligible(const cvvae_conv_desc* d, const char** why) {
   const cvvae_tensor5& x = d->x;
@@ -767,10 +700,8 @@ bool conv_tc_eligible(const cvvae_conv_desc* d, const char** why) {
     if (why) *why = m;
     return false;
   };
-  if (x.s_c != 1) return fail("input channel stride != 1");
+  if (!tma_view(x, elem_bytes(d->dtype))) return fail("input is not a 16-byte aligned channels-last view");
   if (d->w_ld % 8 != 0 || (d->w_ld == 0 && x.C % 8 != 0)) return fail("weight row stride not a 16-byte multiple");
-  if ((x.s_w % 8) || (x.s_h % 8) || (x.s_t % 8) || (x.s_b % 8)) return fail("input strides not 16-byte multiples");
-  if (reinterpret_cast<uintptr_t>(x.ptr) % 16) return fail("input pointer not 16-byte aligned");
   if (reinterpret_cast<uintptr_t>(d->w) % 16) return fail("weight pointer not 16-byte aligned");
   if (d->pad_hw != CVVAE_PAD_ZERO) {
     // replicate padding in H/W is only needed when a tap can actually leave the image
@@ -804,23 +735,6 @@ static int launch_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUten
   return CVVAE_OK;
 }
 
-// Byte strides of y's W, H, T and B axes for a tensor map, or false when TMA cannot address y: channel stride != 1, or a
-// pointer or stride that is not a multiple of 16 bytes.  An axis of extent 1 may carry any stride; it gets a valid one.
-static bool y_map_strides(const cvvae_tensor5& y, int esz, cuuint64_t* strides) {
-  const long long s[4] = {y.s_w, y.s_h, y.s_t, y.s_b};
-  const int n[4] = {y.W, y.H, y.T, y.B};
-  if (y.s_c != 1 || reinterpret_cast<uintptr_t>(y.ptr) % 16) return false;
-  for (int i = 0; i < 4; ++i) {
-    if (n[i] == 1) {
-      strides[i] = (static_cast<cuuint64_t>(y.C) * esz + 15) & ~cuuint64_t(15);
-    } else {
-      if (s[i] <= 0 || (s[i] * esz) % 16) return false;
-      strides[i] = static_cast<cuuint64_t>(s[i]) * esz;
-    }
-  }
-  return true;
-}
-
 // The output goes through shared memory and TMA stores (and the residual comes in by TMA) when y is a 16-bit channels-last
 // tensor TMA can address, with the residual on the same strides and a block of 64 channels staged per A-ring slot (the
 // BN / 64 blocks need that many slots; a slot always holds one, since slab_rows >= TH).  fp32 outputs (logits, fp32
@@ -829,9 +743,9 @@ static bool tma_epilogue_ok(const cvvae_conv_desc* d, const ConvTcParams& p) {
   const char* env = getenv("CVVAE_TMA_EPILOGUE");
   if (env && strcmp(env, "0") == 0) return false;
   if (d->dtype == CVVAE_F32 || (d->flags & (CVVAE_CONV_OUT_F32 | CVVAE_CONV_BIAS_ALONG_M))) return false;
-  cuuint64_t strides[4];
-  if (!y_map_strides(d->y, 2, strides)) return false;
-  if (d->residual && reinterpret_cast<uintptr_t>(d->residual) % 16) return false;
+  cvvae_tensor5 r = d->y;   // the residual shares y's strides
+  r.ptr = const_cast<void*>(d->residual);
+  if (!tma_view(d->y, 2) || (d->residual && !tma_view(r, 2))) return false;
   if (p.Cout % 8 || (p.up_time == 2 && (p.Cout / 2) % 64)) return false;
   return p.N_cta / 64 <= p.NA;
 }
@@ -974,29 +888,12 @@ int conv_tc_launch(const cvvae_conv_desc* d, cudaStream_t stream) {
   // ---- tensor maps
   CUtensorMap tmA, tmB;
   {
-    cuuint64_t dims[5] = {(cuuint64_t)x.C, (cuuint64_t)x.W, (cuuint64_t)x.H, (cuuint64_t)x.T, (cuuint64_t)x.B};
-    cuuint64_t strides[4] = {(cuuint64_t)x.s_w * esz, (cuuint64_t)x.s_h * esz, (cuuint64_t)x.s_t * esz, (cuuint64_t)x.s_b * esz};
-    // degenerate dims may carry meaningless strides; TMA wants multiples of 16 and monotone-ish validity
-    for (int i = 0; i < 4; ++i)
-      if (dims[i + 1] == 1 && (strides[i] == 0 || strides[i] % 16)) strides[i] = (cuuint64_t)x.C * esz;
-    cuuint32_t box[5], estr[5] = {1, (cuuint32_t)d->sw, (cuuint32_t)d->sh, 1, 1};
-    box[0] = (cuuint32_t)cb;
-    if (p.flat) {
-      box[1] = 128; box[2] = 1;
-    } else {
-      box[1] = (cuuint32_t)(p.TW * d->sw);
-      box[2] = (cuuint32_t)(p.slab_rows * d->sh);
-    }
-    box[3] = 1; box[4] = 1;
-    if (!encode_map(&tmA, x.ptr, 5, dims, strides, box, estr, esz)) return CVVAE_E_CUDA;
-  }
-  {
+    const cuuint32_t box[5] = {(cuuint32_t)cb, (cuuint32_t)(p.flat ? 128 : p.TW * d->sw), (cuuint32_t)(p.flat ? 1 : p.slab_rows * d->sh), 1, 1},
+                     estr[5] = {1, (cuuint32_t)d->sw, (cuuint32_t)d->sh, 1, 1};
     const int taps = (d->flags & CVVAE_CONV_W_PER_BATCH) ? x.B > y.B ? x.B : y.B : d->KT * d->KH * d->KW;
-    cuuint64_t dims[3] = {(cuuint64_t)p.Cin, (cuuint64_t)p.Cout, (cuuint64_t)taps};
-    const cuuint64_t wld = d->w_ld ? (cuuint64_t)d->w_ld : (cuuint64_t)p.Cin;
-    cuuint64_t strides[2] = {wld * esz, wld * p.Cout * esz};
-    cuuint32_t box[3] = {(cuuint32_t)cb, (cuuint32_t)N_cta, 1}, estr[3] = {1, 1, 1};
-    if (!encode_map(&tmB, d->w, 3, dims, strides, box, estr, esz)) return CVVAE_E_CUDA;
+    if (!act_map(&tmA, x, esz, box, estr) ||
+        !weight_map(&tmB, d->w, p.Cin, p.Cout, taps, d->w_ld ? d->w_ld : p.Cin, esz, cb, N_cta))
+      return CVVAE_E_CUDA;
   }
 
   // ---- fused 1x1 shortcut: a second input tensor (same positions as the output) and a [Cout][Cin2] matrix
@@ -1007,8 +904,7 @@ int conv_tc_launch(const cvvae_conv_desc* d, cudaStream_t stream) {
     const cvvae_tensor5& x2 = d->x2;
     CVVAE_CHECK_ARG(tensor_ok(&x2) && x2.B == y.B && x2.T == y.T && x2.H == y.H && x2.W == y.W,
                     "conv: fused shortcut input must have the output's [B,T,H,W] extents");
-    CVVAE_CHECK_ARG(x2.s_c == 1 && x2.C % 8 == 0 && !(x2.s_w % 8) && !(x2.s_h % 8) && !(x2.s_t % 8) && !(x2.s_b % 8) &&
-                        reinterpret_cast<uintptr_t>(x2.ptr) % 16 == 0 && reinterpret_cast<uintptr_t>(d->w2) % 16 == 0,
+    CVVAE_CHECK_ARG(tma_view(x2, esz) && x2.C % 8 == 0 && reinterpret_cast<uintptr_t>(d->w2) % 16 == 0,
                     "conv: fused shortcut operands must be 16-byte aligned channels-last views with C %% 8 == 0");
     CVVAE_CHECK_ARG(!p.flat && p.up_time == 1 && d->st == 1 && d->sh == 1 && d->sw == 1 && !d->residual &&
                         !(d->flags & (CVVAE_CONV_BIAS_ALONG_M | CVVAE_CONV_OUT_F32 | CVVAE_CONV_W_PER_BATCH | CVVAE_CONV_X_SHARED)),
@@ -1017,20 +913,9 @@ int conv_tc_launch(const cvvae_conv_desc* d, cudaStream_t stream) {
                     "conv: fused shortcut needs the centre tap inside the kernel window");
     p.Cin2 = x2.C;
     p.cblocks2 = (x2.C + cb - 1) / cb;
-    {
-      cuuint64_t dims[5] = {(cuuint64_t)x2.C, (cuuint64_t)x2.W, (cuuint64_t)x2.H, (cuuint64_t)x2.T, (cuuint64_t)x2.B};
-      cuuint64_t strides[4] = {(cuuint64_t)x2.s_w * esz, (cuuint64_t)x2.s_h * esz, (cuuint64_t)x2.s_t * esz, (cuuint64_t)x2.s_b * esz};
-      for (int i = 0; i < 4; ++i)
-        if (dims[i + 1] == 1 && (strides[i] == 0 || strides[i] % 16)) strides[i] = (cuuint64_t)x2.C * esz;
-      cuuint32_t box[5] = {(cuuint32_t)cb, (cuuint32_t)p.TW, (cuuint32_t)p.slab_rows, 1, 1}, estr[5] = {1, 1, 1, 1, 1};
-      if (!encode_map(&tmA2, x2.ptr, 5, dims, strides, box, estr, esz)) return CVVAE_E_CUDA;
-    }
-    {
-      cuuint64_t dims[3] = {(cuuint64_t)x2.C, (cuuint64_t)p.Cout, 1};
-      cuuint64_t strides[2] = {(cuuint64_t)x2.C * esz, (cuuint64_t)x2.C * p.Cout * esz};
-      cuuint32_t box[3] = {(cuuint32_t)cb, (cuuint32_t)N_cta, 1}, estr[3] = {1, 1, 1};
-      if (!encode_map(&tmB2, d->w2, 3, dims, strides, box, estr, esz)) return CVVAE_E_CUDA;
-    }
+    const cuuint32_t box[5] = {(cuuint32_t)cb, (cuuint32_t)p.TW, (cuuint32_t)p.slab_rows, 1, 1}, estr[5] = {1, 1, 1, 1, 1};
+    if (!act_map(&tmA2, x2, esz, box, estr) || !weight_map(&tmB2, d->w2, x2.C, p.Cout, 1, x2.C, esz, cb, N_cta))
+      return CVVAE_E_CUDA;
   }
 
   // fused GroupNorm statistics need power-of-two channels per group and one sample per CTA index
@@ -1051,14 +936,12 @@ int conv_tc_launch(const cvvae_conv_desc* d, cudaStream_t stream) {
   // ---- TMA epilogue: y and the residual (same strides) as 5-D maps, one box = 64 positions x 64 channels
   CUtensorMap tmY = tmA, tmR = tmA;
   if (p.tma_epi) {
-    cuuint64_t dims[5] = {(cuuint64_t)y.C, (cuuint64_t)y.W, (cuuint64_t)y.H, (cuuint64_t)y.T, (cuuint64_t)y.B};
-    cuuint64_t strides[4];
-    y_map_strides(y, esz, strides);
     const bool rows = p.ROWS >= 2;
-    cuuint32_t box[5] = {(cuuint32_t)cb, (cuuint32_t)(rows ? p.TW : 64), (cuuint32_t)(rows ? p.ROWS / 2 : 1), 1, 1},
-               estr[5] = {1, 1, 1, 1, 1};
-    if (!encode_map(&tmY, y.ptr, 5, dims, strides, box, estr, esz)) return CVVAE_E_CUDA;
-    if (d->residual && !encode_map(&tmR, d->residual, 5, dims, strides, box, estr, esz)) return CVVAE_E_CUDA;
+    const cuuint32_t box[5] = {(cuuint32_t)cb, (cuuint32_t)(rows ? p.TW : 64), (cuuint32_t)(rows ? p.ROWS / 2 : 1), 1, 1},
+                     estr[5] = {1, 1, 1, 1, 1};
+    cvvae_tensor5 r = y;   // the residual shares y's strides
+    r.ptr = const_cast<void*>(d->residual);
+    if (!act_map(&tmY, y, esz, box, estr) || (d->residual && !act_map(&tmR, r, esz, box, estr))) return CVVAE_E_CUDA;
   }
 
   int rc = CVVAE_OK;

@@ -69,6 +69,26 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
+// Cursor over a ring of n buffers guarded by full / empty mbarriers: the slot of the current step and the parity its
+// full barrier completes with (the empty barrier is waited on with the opposite parity).
+struct Ring {
+  uint32_t phase = 0;
+  int slot = 0;
+  __device__ __forceinline__ void advance(int n) {
+    if (++slot == n) {
+      slot = 0;
+      phase ^= 1;
+    }
+  }
+  // the cursor k < n steps on
+  __device__ __forceinline__ Ring ahead(int k, int n) const {
+    Ring r;
+    r.slot = slot + k < n ? slot + k : slot + k - n;
+    r.phase = slot + k < n ? phase : phase ^ 1;
+    return r;
+  }
+};
+
 // ------------------------------------------------------------------ TMA
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];\n" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");

@@ -18,7 +18,6 @@ All arithmetic goes through an ``ops`` backend (``cvvae_b200.ops.CudaOps`` in pr
 """
 from __future__ import annotations
 
-import os
 from dataclasses import dataclass
 from typing import Dict, Optional, Tuple
 
@@ -157,8 +156,9 @@ class Engine:
         self._stats_arena = None   # [slots, B, groups, 2] int64, zeroed once per network pass
         self._stats_next = 0
         self.attn_scratch_bytes = 4 << 30  # cap of the fp32 logits buffer (with fp32 P: logits + P) of the batched spatial attention
-        # 1x1 shortcuts as extra K steps of conv2 (CVVAE_FUSE_SHORTCUT=0: separate launch + residual add, for A/B runs)
-        self.fuse_shortcut = os.environ.get("CVVAE_FUSE_SHORTCUT", "1") != "0"
+        # 1x1 shortcuts as extra K steps of conv2; False runs them as a separate launch + residual add (the form a test
+        # compares the fused one against)
+        self.fuse_shortcut = True
 
     # ------------------------------------------------------------------ shape arithmetic
     def encoded_frames(self, T: int) -> int:

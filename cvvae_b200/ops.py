@@ -148,23 +148,29 @@ class CudaOps:
         mn = 2 * B * t_conv * out.shape[2] * out.shape[3] * Co * Ci
         if k_alg is not None:   # tap-packed network-input conv: count the algorithmic K (taps x real channels), not the padded one
             mn, kt, kh, kw, ref_taps = 2 * B * t_conv * out.shape[2] * out.shape[3] * Co, k_alg, 1, 1, None
-        self.profile["flops"][path] += mn * kt * kh * kw
-        self.profile["ref_flops"][path] += mn * (ref_taps if ref_taps is not None else kt * kh * kw)
+        flops = mn * kt * kh * kw
+        ref_flops = mn * (ref_taps if ref_taps is not None else kt * kh * kw)
+        # algorithmic bytes: every operand once (input, weights, residual, output)
+        nbytes = (x.numel() * x.element_size() + w.numel() * w.element_size() +
+                  out.numel() * out.element_size() * (2 if residual is not None else 1))
         if sc_w is not None:   # the fused 1x1 shortcut's MACs (a separate conv in the reference) and its input bytes
             sc = 2 * B * t_conv * out.shape[2] * out.shape[3] * Co * sc_x.shape[4]
-            self.profile["flops"][path] += sc
-            self.profile["ref_flops"][path] += sc
-            self.profile["bytes"][path] += sc_x.numel() * sc_x.element_size() + sc_w.numel() * sc_w.element_size()
-        # algorithmic bytes: every operand once (input, weights, residual, output)
-        self.profile["bytes"][path] += (x.numel() * x.element_size() + w.numel() * w.element_size() +
-                                        out.numel() * out.element_size() * (2 if residual is not None else 1))
-        self.profile["launches"][path] += 1
+            flops += sc
+            ref_flops += sc
+            nbytes += sc_x.numel() * sc_x.element_size() + sc_w.numel() * sc_w.element_size()
+        self._profiled(path, flops, ref_flops, nbytes, fn, d, x)
+        return out
+
+    def _profiled(self, path: str, flops: int, ref_flops: int, nbytes: int, fn, d: L.ConvDesc, x: torch.Tensor) -> None:
+        """Launch ``fn`` on ``d`` while profiling: add one launch and its counts to ``path``, timed by a CUDA event pair."""
+        prof = self.profile
+        for key, n in (("flops", flops), ("ref_flops", ref_flops), ("bytes", nbytes), ("launches", 1)):
+            prof[key][path] += n
         s_ev, e_ev = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         s_ev.record()
-        L.check(fn(C.byref(d), _stream(x)), "cvvae_conv3d")
+        L.check(fn(C.byref(d), _stream(x)), fn.__name__)
         e_ev.record()
-        self.profile["events"][path].append((s_ev, e_ev))
-        return out
+        prof["events"][path].append((s_ev, e_ev))
 
     @_on_tensor_device
     def conv_tc_plan(self, x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], *, epilogue: bool = False,
@@ -243,20 +249,12 @@ class CudaOps:
         d.up_time = 1
         d.dtype = dtype_code(x.dtype)
         d.alpha = 1.0
-        if self.profile is not None:
-            B, T, H, W, Ci = x.shape
-            fl = 2 * B * out.shape[1] * out.shape[2] * out.shape[3] * cout * Ci * kt * 9
-            self.profile["flops"]["conv_tc"] += fl
-            self.profile["ref_flops"]["conv_tc"] += fl
-            self.profile["bytes"]["conv_tc"] += x.numel() * x.element_size() + out.numel() * out.element_size()
-            self.profile["launches"]["conv_tc"] += 1
-            s_ev, e_ev = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            s_ev.record()
-            L.check(self.lib.cvvae_conv3d_stacked(C.byref(d), _stream(x)), "cvvae_conv3d_stacked")
-            e_ev.record()
-            self.profile["events"]["conv_tc"].append((s_ev, e_ev))
+        fn = self.lib.cvvae_conv3d_stacked
+        if self.profile is None:
+            L.check(fn(C.byref(d), _stream(x)), "cvvae_conv3d_stacked")
         else:
-            L.check(self.lib.cvvae_conv3d_stacked(C.byref(d), _stream(x)), "cvvae_conv3d_stacked")
+            fl = 2 * x.shape[0] * out.shape[1] * out.shape[2] * out.shape[3] * cout * x.shape[4] * kt * 9
+            self._profiled("conv_tc", fl, fl, x.numel() * x.element_size() + out.numel() * out.element_size(), fn, d, x)
         return out
 
     # ------------------------------------------------------------------ normalisation

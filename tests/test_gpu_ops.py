@@ -220,6 +220,85 @@ def test_conv_direct_network_inputs():
         torch.testing.assert_close(got.float(), want, **_tol(torch.float16))
 
 
+def _conv_dispatched_and_direct(ops, x, w, bias, yshape, edit=None, **kw):
+    """One descriptor through cvvae_conv3d and through cvvae_conv3d_direct; ``edit(d)`` may rewrite its input view
+    (strides torch cannot express).  Returns (dispatched output, direct output, cvvae_conv3d_is_tc)."""
+    import ctypes as C
+
+    from cvvae_b200 import _lib as L
+    outs = []
+    for fn in (ops.lib.cvvae_conv3d, ops.lib.cvvae_conv3d_direct):
+        y = torch.zeros(yshape, dtype=x.dtype, device=DEV)
+        d = ops._conv_desc(x, w, bias, out=y, **kw)
+        if edit:
+            edit(d)
+        is_tc = ops.lib.cvvae_conv3d_is_tc(C.byref(d))
+        L.check(fn(C.byref(d), torch.cuda.current_stream().cuda_stream), "conv")
+        outs.append(y)
+    torch.cuda.synchronize()
+    return outs[0], outs[1], is_tc
+
+
+def test_conv_view_with_zero_or_negative_stride_runs_direct():
+    """TMA cannot address an axis of extent > 1 whose stride is zero (a broadcast frame) or negative (frames in reverse
+    order): the dispatcher sends such a view to conv_direct, which reads any strides."""
+    ops, fake = _ops(), FakeOps()
+    base = _rand((1, 4, 12, 16, 64), torch.float16, 40)
+    w = _rand((27, 64, 64), torch.float16, 41, scale=(27 * 64) ** -0.5 * 2)
+    bias = _rand((64,), torch.float32, 42, 0.3)
+    kw = dict(kernel=(3, 3, 3), offset=(-1, -1, -1))
+    yshape = (1, 4, 12, 16, 64)
+
+    def reverse_frames(d):   # base's frames last to first, on the descriptor (torch has no negative strides)
+        d.x.ptr += 3 * d.x.s_t * base.element_size()
+        d.x.s_t = -d.x.s_t
+
+    for x, logical, edit in ((base[:, :1].expand(yshape), base[:, :1].expand(yshape), None),
+                             (base, base.flip(1), reverse_frames)):
+        got, direct, is_tc = _conv_dispatched_and_direct(ops, x, w, bias, yshape, edit, **kw)
+        assert is_tc == 0
+        assert torch.equal(got, direct)
+        want = fake.conv(logical, w, bias, out=torch.zeros(yshape, dtype=torch.float32, device=DEV), **kw)
+        torch.testing.assert_close(got.float(), want, **_tol(torch.float16))
+
+
+def test_conv_view_with_unaligned_stride_on_extent_one_axis_runs_tc():
+    """An axis of extent 1 is never stepped along, so its stride may be anything: a single-frame, single-sample view
+    whose T and B strides are not 16-byte multiples still runs on the tensor cores, bit for bit as its contiguous copy."""
+    ops = _ops()
+    H, W, Ci = 12, 16, 64
+    buf = _rand((H * W * Ci + 16,), torch.float16, 43)
+    x = buf.as_strided((1, 1, H, W, Ci), (5, 3, W * Ci, Ci, 1))
+    w = _rand((9, 64, Ci), torch.float16, 44, scale=(9 * Ci) ** -0.5 * 2)
+    bias = _rand((64,), torch.float32, 45, 0.3)
+    kw = dict(kernel=(1, 3, 3), offset=(0, -1, -1))
+    yshape = (1, 1, H, W, 64)
+    got, direct, is_tc = _conv_dispatched_and_direct(ops, x, w, bias, yshape, **kw)
+    assert is_tc == 1
+    torch.testing.assert_close(got.float(), direct.float(), **_tol(torch.float16))
+    same = ops.conv(x.contiguous(), w, bias, out=torch.zeros(yshape, dtype=torch.float16, device=DEV), force="tc", **kw)
+    torch.cuda.synchronize()
+    assert torch.equal(got, same)
+
+
+def test_conv_fp32_view_with_16_byte_position_stride_runs_tc():
+    """TMA needs 16-byte strides, not 8-element ones: an fp32 view 32 channels wide in rows of 36 floats (144 bytes, a
+    stride of 4 mod 8 elements) runs on the tensor cores, bit for bit as its contiguous copy."""
+    ops = _ops()
+    x = _rand((1, 2, 12, 16, 36), torch.float32, 46)[..., :32]
+    assert x.stride(3) % 8 == 4
+    w = ops.pack_weight(_rand((32, 32, 1, 3, 3), torch.float32, 47, scale=(9 * 32) ** -0.5 * 2))
+    bias = _rand((32,), torch.float32, 48, 0.3)
+    kw = dict(kernel=(1, 3, 3), offset=(0, -1, -1))
+    yshape = (1, 2, 12, 16, 32)
+    got, direct, is_tc = _conv_dispatched_and_direct(ops, x, w, bias, yshape, **kw)
+    assert is_tc == 1
+    torch.testing.assert_close(got, direct, rtol=1e-2, atol=1e-2)   # TF32 products against fp32 ones
+    same = ops.conv(x.contiguous(), w, bias, out=torch.zeros(yshape, dtype=torch.float32, device=DEV), force="tc", **kw)
+    torch.cuda.synchronize()
+    assert torch.equal(got, same)
+
+
 def test_conv_attention_style_gemms():
     """fp32 logits with a ragged token count, bias along rows, weight row stride (the three attention GEMMs)."""
     ops, fake = _ops(), FakeOps()

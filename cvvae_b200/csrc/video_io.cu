@@ -96,9 +96,95 @@ __global__ void __launch_bounds__(256) resize_u8_kernel(const uint8_t* __restric
   }
 }
 
+// One axis of torchvision's antialiased bilinear resize of a *float* tensor, as ATen's CPU kernel evaluates it
+// (UpSampleKernel.cpp, _compute_indices_min_size_weights_aa with a float scalar type): centre c = scale * (i + 0.5) rounded
+// to float, support s = max(scale, 1), window [int(c - s + 0.5), int(c + s + 0.5)) clipped to the input and to at most
+// 2 * ceil(s) + 1 taps, triangle weights 1 - |(j - c + 0.5) * invscale| normalised by their float sum.  The `+ 0.5` and the
+// product with invscale are double there (a float plus a double literal), so they are double here too, and every rounding
+// ATen makes in fp32 is made here: the windows are the CPU kernel's and the weights differ from its by rounding order only.
+struct AaAxis {
+  float center, invscale, total;
+  int lo, n;
+  __device__ __forceinline__ AaAxis(int i, int in_size, float scale) {
+    const float support = scale >= 1.f ? scale : 1.f;
+    invscale = scale >= 1.f ? 1.f / scale : 1.f;
+    // the double product of ATen is exact, so one rounding either way; the _rn intrinsics keep the compiler from fusing
+    // the centre's product into the subtractions below (an unrounded centre moves windows and weights)
+    center = __fmul_rn(scale, static_cast<float>(i) + 0.5f);
+    lo = max(0, static_cast<int>(static_cast<double>(__fsub_rn(center, support)) + 0.5));
+    n = min(in_size, static_cast<int>(static_cast<double>(__fadd_rn(center, support)) + 0.5)) - lo;
+    n = min(max(n, 0), static_cast<int>(ceilf(support)) * 2 + 1);
+    total = 0.f;
+    for (int j = 0; j < n; ++j) total += raw(j);
+  }
+  __device__ __forceinline__ float raw(int j) const {
+    const float d = __fsub_rn(static_cast<float>(j + lo), center);
+    return fmaxf(0.f, 1.f - fabsf(static_cast<float>(__dmul_rn(__dadd_rn(d, 0.5), invscale))));
+  }
+  __device__ __forceinline__ float weight(int j) const { return total != 0.f ? raw(j) / total : raw(j); }
+};
+
+// The reference's training pre-processing of uint8 frames [T,H,W,3] (lvdm/data/decoder.py:99-109, transform.py): to float,
+// antialiased bilinear resize to RH x RW, crop of OH x OW at (top, left), then (v / 255 - 0.5) * 2, all fp32, rounded once
+// to the output type.  Output pixel (t, oy, ox) is pixel (oy + top, ox + left) of the resized frame, so the crop costs
+// nothing.  Width is reduced first, then height, as ATen's separable kernel does (an axis whose size does not change gets
+// the weights {1, 0}, which leaves it exact, as ATen's skipping of that axis does).  One thread per output pixel.
+template <int DT>
+__global__ void __launch_bounds__(256) train_input_kernel(const uint8_t* __restrict__ in, typename Elem<DT>::T* __restrict__ out,
+                                                          int T, int H, int W, int top, int left, int OH, int OW, float sh,
+                                                          float sw) {
+  using E = Elem<DT>;
+  const long long n = 1ll * T * OH * OW;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int ox = static_cast<int>(i % OW);
+    const int oy = static_cast<int>((i / OW) % OH);
+    const int t = static_cast<int>(i / (1ll * OW * OH));
+    const AaAxis ay(oy + top, H, sh), ax(ox + left, W, sw);
+    const uint8_t* base = in + ((1ll * t * H + ay.lo) * W + ax.lo) * 3;
+    float acc0 = 0.f, acc1 = 0.f, acc2 = 0.f;
+    for (int b = 0; b < ay.n; ++b) {
+      const uint8_t* rowp = base + 1ll * b * W * 3;
+      float r0 = 0.f, r1 = 0.f, r2 = 0.f;
+      for (int a = 0; a < ax.n; ++a) {
+        const float wx = ax.weight(a);
+        r0 = fmaf(wx, static_cast<float>(rowp[a * 3 + 0]), r0);
+        r1 = fmaf(wx, static_cast<float>(rowp[a * 3 + 1]), r1);
+        r2 = fmaf(wx, static_cast<float>(rowp[a * 3 + 2]), r2);
+      }
+      const float wy = ay.weight(b);
+      acc0 = fmaf(wy, r0, acc0);
+      acc1 = fmaf(wy, r1, acc1);
+      acc2 = fmaf(wy, r2, acc2);
+    }
+    const float v[3] = {acc0, acc1, acc2};
+#pragma unroll
+    for (int c = 0; c < 3; ++c) out[1ll * c * n + i] = E::from_f((v[c] / 255.f - 0.5f) * 2.f);
+  }
+}
+
 }  // namespace cvvae
 
 using namespace cvvae;
+
+extern "C" int cvvae_video_train_input(const uint8_t* thwc, void* out_cthw, int32_t T, int32_t H, int32_t W, int32_t RH,
+                                       int32_t RW, int32_t top, int32_t left, int32_t OH, int32_t OW, int32_t dtype,
+                                       void* stream) {
+  CVVAE_CHECK_ARG(thwc && out_cthw && T > 0 && H > 0 && W > 0 && RH > 0 && RW > 0 && OH > 0 && OW > 0,
+                  "cvvae_video_train_input: bad argument (T=%d H=%d W=%d RH=%d RW=%d OH=%d OW=%d)", T, H, W, RH, RW, OH, OW);
+  CVVAE_CHECK_ARG(top >= 0 && left >= 0 && 1ll * top + OH <= RH && 1ll * left + OW <= RW,
+                  "cvvae_video_train_input: crop %dx%d at (%d, %d) does not lie inside the %dx%d resized frame", OH, OW, top,
+                  left, RH, RW);
+  const long long n = 1ll * T * OH * OW;
+  const unsigned blocks = static_cast<unsigned>(n / 256 + 1 < 16ll * num_sms() ? n / 256 + 1 : 16ll * num_sms());
+  const float sh = static_cast<float>(H) / static_cast<float>(RH), sw = static_cast<float>(W) / static_cast<float>(RW);
+  CVVAE_DISPATCH_DTYPE(dtype, {
+    train_input_kernel<DT><<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        thwc, reinterpret_cast<typename Elem<DT>::T*>(out_cthw), T, H, W, top, left, OH, OW, sh, sw);
+  });
+  CVVAE_LAUNCH_CHECK();
+  return CVVAE_OK;
+}
 
 extern "C" int cvvae_video_resize_u8(const uint8_t* thwc, uint8_t* out_thwc, void* out_cthw, int32_t T, int32_t H, int32_t W,
                                      int32_t OH, int32_t OW, int32_t dtype, void* stream) {

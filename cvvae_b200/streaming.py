@@ -12,6 +12,10 @@ chunk however long the clip is, and the concatenated chunks are bit-identical to
 ``reconstruct_frames`` chains pixel upload, encoder, posterior, decoder and pixel download over host uint8 frames:
 the body of the reference's ``cvvae_inference_video.py`` as a stream.  ``evaluate_frames`` is the same stream with every
 reconstructed frame scored (PSNR, SSIM) on the device against the input frame the network saw.
+
+``encode_clips`` turns a dataset of clips into latents: each clip goes through the reference's training pre-processing
+(``video_io.frames_to_training_input``) straight into its slot of a batch, and batches of clips with equal length run
+through one ``model.encode`` call each.
 """
 from __future__ import annotations
 
@@ -306,3 +310,119 @@ def _reconstruct(model, enc: StreamEncoder, dec: StreamDecoder, frames: Iterator
     refs.clear()   # the trailing frames that were never reconstructed
     while downloads:
         yield piece()
+
+
+def clip_batches(clips: Iterable, batch_size: int, length=len) -> Iterator[list]:
+    """The batching schedule of ``encode_clips``: consecutive clips of equal ``length(clip)`` in batches of at most
+    `batch_size`, in input order.  A batch closes as soon as it is full, when a clip of another length arrives, or at the
+    end of the input; it is yielded then, before the next clip is read."""
+    batch: list = []
+    for clip in clips:
+        if batch and length(clip) != length(batch[0]):
+            yield batch
+            batch = []
+        batch.append(clip)
+        if len(batch) == batch_size:
+            yield batch
+            batch = []
+    if batch:
+        yield batch
+
+
+def encode_clips(model, clips: Iterable, size, resize: str = "cover", batch_size: int = 8) -> Iterator[torch.Tensor]:
+    """Encode a dataset of clips to latent moments, batched on the GPU.
+
+    `clips` is an iterable of host uint8 clips ``[T, H, W, 3]`` (numpy arrays or CPU tensors; T >= 1, a 1-frame clip is
+    an image; T and the source size may differ from clip to clip).  Yields, for each clip in input order, a host tensor
+    ``[2 z, t', h', w']`` in the model's dtype equal bit for bit to::
+
+        model.encode(frames_to_training_input(clip.cuda(), size, resize, model.dtype)).latent_dist.parameters[0]
+
+    that is, the clip prepared as the reference's training data path prepares it (``video_io.training_geometry``:
+    "cover" = CoverResize + CenterCrop, "short" = Resize(min(size)) + CenterCrop), then encoded.
+    ``DiagonalGaussianDistribution(moments[None])`` gives ``mode()`` / ``sample()``.
+
+    Consecutive clips of equal T are stacked into one ``[B, 3, T, h, w]`` input (B <= `batch_size`, see
+    ``clip_batches``), each clip written into its slot by one kernel launch, and the batch runs through one
+    ``model.encode`` call, with the model's chunking, tiling and CUDA graphs.  Batching does not change any clip's
+    moments: the engine's tile plans and GroupNorm statistics are per sample.
+
+    Uploads and downloads run on a side stream, overlapped with the kernels on the device's current stream, and a batch's
+    moments are yielded once the next batch has been enqueued.  Device memory holds one batch's input, activations and
+    moments plus the source frames of the clips in flight, however many clips there are.  Yielded tensors are the
+    caller's: later yields never overwrite them.
+
+    Raises ValueError at the call for a model that is not on CUDA, `batch_size` < 1 or a malformed `size` / `resize`,
+    and when an item arrives that is not a host uint8 ``[T, H, W, 3]`` clip with T >= 1, or whose centre crop torchvision
+    would pad.
+    """
+    from .video_io import _check_resize, _check_size
+    if model.device.type != "cuda":
+        raise ValueError("encode_clips: the model must be on a CUDA device")
+    if isinstance(batch_size, bool) or not isinstance(batch_size, int) or batch_size < 1:
+        raise ValueError(f"encode_clips: batch_size must be an int >= 1; got {batch_size!r}")
+    size = _check_size(size)
+    _check_resize(resize)
+    return _encode_clips(model, iter(clips), size, resize, batch_size)
+
+
+def _encode_clips(model, clips: Iterator, size: tuple, resize: str, batch_size: int) -> Iterator[torch.Tensor]:
+    from .video_io import frames_to_training_input, training_geometry
+
+    def checked(items):
+        for item in items:
+            item = torch.as_tensor(item)
+            if (item.dtype != torch.uint8 or item.dim() != 4 or item.shape[0] < 1 or item.shape[-1] != 3
+                    or item.device.type != "cpu"):
+                raise ValueError("encode_clips expects host uint8 clips [T, H, W, 3] with T >= 1; "
+                                 f"got {item.dtype} {tuple(item.shape)} on {item.device}")
+            training_geometry(item.shape[1], item.shape[2], size, resize)   # refuses a crop torchvision would pad
+            yield item
+
+    # As in _reconstruct, no device context is held across the yields: every allocation, stream and launch names the
+    # model's device, and the kernels run on that device's current stream.
+    dev = model.device
+    copy = torch.cuda.Stream(device=dev)
+    staging: Optional[torch.Tensor] = None   # pinned upload buffer (flat), refilled once its last upload has completed
+    staged = torch.cuda.Event()
+    downloads: deque = deque()               # (host moments [B, 2z, t', h', w'], event of their download), oldest first
+
+    def results():
+        host, done = downloads.popleft()
+        done.synchronize()
+        return list(host.unbind(0))
+
+    for batch in clip_batches(checked(clips), batch_size):
+        compute = torch.cuda.current_stream(dev)
+        x = torch.empty((len(batch), 3, batch[0].shape[0], *size), dtype=model.dtype, device=dev)
+        for i, clip in enumerate(batch):
+            # host -> pinned staging -> device on the copy stream; the compute stream waits for that upload only
+            staged.synchronize()
+            if staging is None or staging.numel() < clip.numel():
+                staging = torch.empty(clip.numel(), dtype=torch.uint8, pin_memory=True)
+            pinned = staging[:clip.numel()].view(clip.shape)
+            pinned.copy_(clip)
+            with torch.cuda.stream(copy):
+                src = torch.empty(clip.shape, dtype=torch.uint8, device=dev)
+                src.copy_(pinned, non_blocking=True)
+                staged.record(copy)
+            compute.wait_event(staged)
+            src.record_stream(compute)
+            frames_to_training_input(src, size, resize, model.dtype, out=x[i:i + 1])
+            del src
+        moments = model.encode(x).latent_dist.parameters
+        del x
+        host = _pinned(moments.shape, moments)
+        copy.wait_stream(compute)
+        with torch.cuda.stream(copy):
+            host.copy_(moments, non_blocking=True)
+            done = torch.cuda.Event()
+            done.record(copy)
+        moments.record_stream(copy)
+        del moments
+        downloads.append((host, done))
+        # one-batch lag: a batch's moments go to the caller only once the next batch is enqueued behind it
+        while len(downloads) > 1:
+            yield from results()
+    while downloads:
+        yield from results()

@@ -20,8 +20,8 @@
  *     products, fp32 accumulation), as PyTorch's default fp32 convolution does on this GPU.  Outputs whose only
  *     consumers are tensor-core products (packed weights, GroupNorm / LayerNorm / softmax outputs, pack_taps_hw and the
  *     channels-first -> channels-last copy of a network input) are stored rounded to the nearest TF32 value; every other output
- *     (convolution outputs: residual stream, q / k / v, attention output) is full fp32.  The video_io entry points and
- *     cvvae_conv3d_stacked are 16-bit only and reject CVVAE_F32.
+ *     (convolution outputs: residual stream, q / k / v, attention output) is full fp32.  The video_io entry points of the
+ *     inference script and cvvae_conv3d_stacked are 16-bit only and reject CVVAE_F32; cvvae_video_train_input takes all three.
  */
 #ifndef CVVAE_B200_H_
 #define CVVAE_B200_H_
@@ -195,6 +195,15 @@ int cvvae_video_f16_to_u8(const void* in_cthw, uint8_t* thwc, int32_t T, int32_t
  * fp32 arithmetic: within 1 LSB of torchvision's fixed-point uint8 path (differs on < 1 % of the pixels). */
 int cvvae_video_resize_u8(const uint8_t* thwc, uint8_t* out_thwc, void* out_cthw, int32_t T, int32_t H, int32_t W, int32_t OH,
                           int32_t OW, int32_t dtype, void* stream);
+/* The training data path's pre-processing (lvdm/data/decoder.py:99-109, 275-279; lvdm/data/transform.py:14-59, 66-121):
+ * `torch.tensor(frames).permute(0, 3, 1, 2).float()`, `CoverResize(size)` or `Resize(min(size))`, `CenterCrop(size)`,
+ * `(frames / 255 - 0.5) * 2`, as one pass.  uint8 thwc [T,H,W,3] -> out_cthw [3,T,OH,OW] (contiguous, F16 / BF16 / F32):
+ * out(c,t,oy,ox) = pixel (oy + top, ox + left) of the frame resized to RH x RW by torchvision's antialiased bilinear
+ * resize of a float tensor (ATen's CPU windows and weights, width reduced first, fp32 arithmetic, no rounding to uint8),
+ * then (v / 255 - 0.5) * 2 in fp32, rounded once to the output type.  The crop window must lie inside RH x RW, else
+ * CVVAE_E_ARG.  One kernel launch. */
+int cvvae_video_train_input(const uint8_t* thwc, void* out_cthw, int32_t T, int32_t H, int32_t W, int32_t RH, int32_t RW,
+                            int32_t top, int32_t left, int32_t OH, int32_t OW, int32_t dtype, void* stream);
 
 /* Reconstruction quality: per-frame squared error and SSIM of two uint8 videos a, b: [T,H,W,3], contiguous, on the device.
  * They are the two ends of the inference script: its resized uint8 input (cvvae_inference_video.py:28) and the uint8

@@ -5,7 +5,10 @@ There is no CPU fallback: if the shared library is missing or a call fails, an e
 from __future__ import annotations
 
 import ctypes as C
+import functools
 import os
+
+import torch
 
 from ._build import LIBPATH
 
@@ -109,3 +112,31 @@ def check(rc: int, what: str) -> None:
     if rc != 0:
         msg = load().cvvae_last_error().decode(errors="replace")
         raise CvvaeError(f"{what} failed ({rc}): {msg}")
+
+
+def _stream(t: torch.Tensor) -> int:
+    """The handle of the current stream of `t`'s device, which the library launches on."""
+    return torch.cuda.current_stream(t.device).cuda_stream
+
+
+def _on_tensor_device(fn):
+    """Run `fn` (a function or a method) with the CUDA device of its first tensor argument current.
+
+    The C ABI launches on the current device (kernel attributes, SM count and the stream handle are per device), so
+    a call on tensors of cuda:1 while cuda:0 is current - single-process multi-GPU, diffusers device placement - must
+    switch for the duration of the call, exactly as a PyTorch operator would.  Host and meta tensors go straight to
+    `fn`, whose own checks refuse them, without initialising CUDA."""
+
+    @functools.wraps(fn)
+    def wrapper(*args, **kwargs):
+        dev = None
+        for a in args:
+            if isinstance(a, torch.Tensor):
+                dev = a.device
+                break
+        if dev is None or dev.type != "cuda" or dev.index == torch.cuda.current_device():
+            return fn(*args, **kwargs)
+        with torch.cuda.device(dev):
+            return fn(*args, **kwargs)
+
+    return wrapper

@@ -32,13 +32,13 @@ class FrameMetrics(NamedTuple):
     sse: torch.Tensor    # int64 [T], sum of squared differences over the frame
 
 
+@L._on_tensor_device
 def _launch(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
     """The kernel on the current stream of the frames' device: int64 [T, 2] (sse, sum of ssim * 2^32), on the device."""
     T, H, W, _ = a.shape
     acc = torch.empty((T, 2), dtype=torch.int64, device=a.device)
-    with torch.cuda.device(a.device):
-        L.check(L.load().cvvae_frame_metrics(a.data_ptr(), b.data_ptr(), T, H, W, acc.data_ptr(),
-                                             torch.cuda.current_stream(a.device).cuda_stream), "cvvae_frame_metrics")
+    L.check(L.load().cvvae_frame_metrics(a.data_ptr(), b.data_ptr(), T, H, W, acc.data_ptr(), L._stream(a)),
+            "cvvae_frame_metrics")
     return acc
 
 

@@ -16,6 +16,7 @@ from typing import Optional, Sequence, Tuple
 import torch
 
 from . import _lib as L
+from ._lib import _on_tensor_device, _stream
 
 _DT = {torch.float16: L.F16, torch.bfloat16: L.BF16, torch.float32: L.F32}
 
@@ -33,35 +34,8 @@ def _t5(t: torch.Tensor) -> L.Tensor5:
     return L.Tensor5(t.data_ptr(), t.shape[0], t.shape[1], t.shape[2], t.shape[3], t.shape[4], s[0], s[1], s[2], s[3], s[4])
 
 
-def _stream(t: torch.Tensor) -> int:
-    return torch.cuda.current_stream(t.device).cuda_stream
-
-
 def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
     return None if t is None else t.data_ptr()
-
-
-def _on_tensor_device(fn):
-    """Run a CudaOps method with the CUDA device of its first tensor argument current.
-
-    The C ABI launches on the current device (kernel attributes, SM count and the stream handle are per device), so
-    a model living on cuda:1 while cuda:0 is current - single-process multi-GPU, diffusers device placement - must
-    switch for the duration of the call, exactly as a PyTorch operator would."""
-    import functools
-
-    @functools.wraps(fn)
-    def wrapper(self, *args, **kwargs):
-        dev = None
-        for a in args:
-            if isinstance(a, torch.Tensor):
-                dev = a.device
-                break
-        if dev is None or dev.type != "cuda" or dev.index == torch.cuda.current_device():
-            return fn(self, *args, **kwargs)
-        with torch.cuda.device(dev):
-            return fn(self, *args, **kwargs)
-
-    return wrapper
 
 
 class CudaOps:

@@ -140,8 +140,72 @@ class StreamDecoder(_ChunkStream):
     _which = "decode"
 
 
-def _pinned(shape, like: torch.Tensor) -> torch.Tensor:
-    return torch.empty(shape, dtype=like.dtype, pin_memory=True)
+def _pinned(shape, dtype: torch.dtype) -> torch.Tensor:
+    return torch.empty(shape, dtype=dtype, pin_memory=True)
+
+
+class _HostTransfers:
+    """The host <-> device copies of one host-facing stream: on a side copy stream of `dev`, overlapped with the kernels
+    on that device's current (compute) stream.  Every allocation and stream names `dev`, so no device context is held
+    between calls, and the callers may yield between them."""
+
+    def __init__(self, dev: torch.device):
+        self._dev = dev
+        self._copy = torch.cuda.Stream(device=dev)
+        self._staging: Optional[torch.Tensor] = None   # pinned uint8, flat, grown on demand; reused once its upload is done
+        self._staged = torch.cuda.Event()
+        self._downloads: deque = deque()               # (host tensors, event of their download), oldest first
+
+    def __len__(self) -> int:
+        """Downloads queued and not yet taken."""
+        return len(self._downloads)
+
+    def upload(self, host_u8: torch.Tensor) -> torch.Tensor:
+        """host -> pinned staging -> device on the copy stream; the compute stream waits for that upload only."""
+        n = host_u8.numel()
+        self._staged.synchronize()
+        if self._staging is None or self._staging.numel() < n:
+            self._staging = _pinned(n, torch.uint8)
+        pinned = self._staging[:n].view(host_u8.shape)
+        pinned.copy_(host_u8)
+        with torch.cuda.stream(self._copy):
+            out = torch.empty(host_u8.shape, dtype=torch.uint8, device=self._dev)
+            out.copy_(pinned, non_blocking=True)
+            self._staged.record(self._copy)
+        compute = torch.cuda.current_stream(self._dev)
+        compute.wait_event(self._staged)
+        out.record_stream(compute)
+        return out
+
+    def download(self, *tensors: torch.Tensor) -> None:
+        """Queue copies of `tensors` into fresh pinned host tensors, made after everything already enqueued on the
+        compute stream."""
+        hosts = tuple(_pinned(t.shape, t.dtype) for t in tensors)
+        self._copy.wait_stream(torch.cuda.current_stream(self._dev))
+        with torch.cuda.stream(self._copy):
+            for host, t in zip(hosts, tensors):
+                host.copy_(t, non_blocking=True)
+            done = torch.cuda.Event()
+            done.record(self._copy)
+        for t in tensors:
+            t.record_stream(self._copy)
+        self._downloads.append((hosts, done))
+
+    def take(self) -> tuple:
+        """The host tensors of the oldest queued download, as passed to ``download``, once its copies have completed."""
+        hosts, done = self._downloads.popleft()
+        done.synchronize()
+        return hosts
+
+
+def _host_frames(item, who: str, min_t: int) -> torch.Tensor:
+    """A host item (numpy array or tensor) as a host uint8 tensor [t, H, W, 3] with t >= `min_t`; ValueError otherwise."""
+    item = torch.as_tensor(item)
+    if (item.dtype != torch.uint8 or item.dim() != 4 or item.shape[0] < min_t or item.shape[-1] != 3
+            or item.device.type != "cpu"):
+        expects = f"clips [T, H, W, 3] with T >= {min_t}" if min_t else "frames [t, H, W, 3]"
+        raise ValueError(f"{who} expects host uint8 {expects}; got {item.dtype} {tuple(item.shape)} on {item.device}")
+    return item
 
 
 def reconstruct_frames(model, frames: Iterable, size=None, sample_posterior: bool = False,
@@ -202,16 +266,13 @@ def _reconstruct(model, enc: StreamEncoder, dec: StreamDecoder, frames: Iterator
     from .video_io import frames_to_input, frames_to_input_and_u8, output_to_frames
 
     # No device context is held across the yields (it would leak into the caller's code): every allocation, stream and
-    # launch below names the model's device, and the networks run on that device's current stream.
-    dev = model.device
+    # launch below names the model's device or switches to it for its own duration, and the networks run on that
+    # device's current stream.
     time_compress = model.encode_n_frames_a_time // model.decode_n_frames_a_time
-    copy = torch.cuda.Stream(device=dev)
-    staging: Optional[torch.Tensor] = None   # pinned upload buffer, refilled once its last upload has completed
-    staged = torch.cuda.Event()
+    io = _HostTransfers(model.device)
     pending: deque = deque()    # input frames on the device, not yet fed: the clip may end before they are kept
     refs: deque = deque()       # score only: uint8 input frames as the network saw them, from the first frame not yet scored
     fed = received = 0
-    downloads: deque = deque()  # (host frames, host int64 sums of their scores or None, event of their download), oldest first
 
     def take_refs(n: int) -> torch.Tensor:
         """The next `n` input frames: decoder chunks return the clip's frames in order, [0, 17) then 16 at a time."""
@@ -227,32 +288,17 @@ def _reconstruct(model, enc: StreamEncoder, dec: StreamDecoder, frames: Iterator
 
     def download(x: torch.Tensor) -> None:
         u8 = output_to_frames(x)
-        host = _pinned(u8.shape, u8)
-        acc = None
-        if score:
-            ref = take_refs(u8.shape[0])
-            if ref.shape != u8.shape:
-                raise ValueError(f"evaluate_frames: the networks return {u8.shape[1]} x {u8.shape[2]} frames for an input of "
-                                 f"{ref.shape[1]} x {ref.shape[2]}, and frames of different sizes cannot be scored; pass "
-                                 "`size=` with a size the networks reproduce (a multiple of their spatial stride)")
-            acc = metrics._launch(ref, u8)
-        sums = _pinned(acc.shape, acc) if score else None
-        copy.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(copy):
-            host.copy_(u8, non_blocking=True)
-            if score:
-                sums.copy_(acc, non_blocking=True)
-            done = torch.cuda.Event()
-            done.record(copy)
-        u8.record_stream(copy)
-        if score:
-            acc.record_stream(copy)
-        downloads.append((host, sums, done))
-
-    def piece():
-        host, sums, done = downloads.popleft()
-        done.synchronize()
         if not score:
+            return io.download(u8)
+        ref = take_refs(u8.shape[0])
+        if ref.shape != u8.shape:
+            raise ValueError(f"evaluate_frames: the networks return {u8.shape[1]} x {u8.shape[2]} frames for an input of "
+                             f"{ref.shape[1]} x {ref.shape[2]}, and frames of different sizes cannot be scored; pass "
+                             "`size=` with a size the networks reproduce (a multiple of their spatial stride)")
+        io.download(u8, metrics._launch(ref, u8))
+
+    def piece(host: torch.Tensor, sums: Optional[torch.Tensor] = None):
+        if sums is None:
             return host
         m = metrics._scores(sums, host.shape[1], host.shape[2])
         return host, m.psnr, m.ssim
@@ -264,31 +310,17 @@ def _reconstruct(model, enc: StreamEncoder, dec: StreamDecoder, frames: Iterator
                 download(x)
 
     for item in frames:
-        item = torch.as_tensor(item)
-        if item.dtype != torch.uint8 or item.dim() != 4 or item.shape[-1] != 3 or item.device.type != "cpu":
-            raise ValueError(f"{'evaluate_frames' if score else 'reconstruct_frames'} expects host uint8 frames "
-                             f"[t, H, W, 3]; got {item.dtype} {tuple(item.shape)} on {item.device}")
+        item = _host_frames(item, "evaluate_frames" if score else "reconstruct_frames", 0)
         t = item.shape[0]
         if t == 0:
             continue
-        # host -> pinned staging -> device on the copy stream; the compute stream waits for that upload only
-        staged.synchronize()
-        if staging is None or staging.shape[0] < t or staging.shape[1:] != item.shape[1:]:
-            staging = _pinned(item.shape, item)
-        staging[:t].copy_(item)
-        with torch.cuda.stream(copy):
-            dev_u8 = torch.empty(item.shape, dtype=torch.uint8, device=dev)
-            dev_u8.copy_(staging[:t], non_blocking=True)
-            staged.record(copy)
-        compute = torch.cuda.current_stream(dev)
-        compute.wait_event(staged)
-        dev_u8.record_stream(compute)
+        dev_u8 = io.upload(item)
         if score:
             x, ref = frames_to_input_and_u8(dev_u8, dtype=model.dtype, size=size)
-            pending.append(x)
             refs.append(ref)
         else:
-            pending.append(frames_to_input(dev_u8, dtype=model.dtype, size=size))
+            x = frames_to_input(dev_u8, dtype=model.dtype, size=size)
+        pending.append(x)
         received += t
         # feed up to the last frame the script keeps so far (1 + (T-1)//4*4): frames past it wait for more input, and
         # are dropped if the clip ends first
@@ -301,15 +333,15 @@ def _reconstruct(model, enc: StreamEncoder, dec: StreamDecoder, frames: Iterator
             decode_chunks(enc.feed(x[:, :, :k]))
             fed += k
         # one-chunk lag: a piece goes to the caller only once a later chunk is enqueued behind it
-        while len(downloads) > 1:
-            yield piece()
+        while len(io) > 1:
+            yield piece(*io.take())
     pending.clear()
     decode_chunks(enc.close())
     for x in dec.close():
         download(x)
     refs.clear()   # the trailing frames that were never reconstructed
-    while downloads:
-        yield piece()
+    while io:
+        yield piece(*io.take())
 
 
 def clip_batches(clips: Iterable, batch_size: int, length=len) -> Iterator[list]:
@@ -371,58 +403,25 @@ def _encode_clips(model, clips: Iterator, size: tuple, resize: str, batch_size: 
 
     def checked(items):
         for item in items:
-            item = torch.as_tensor(item)
-            if (item.dtype != torch.uint8 or item.dim() != 4 or item.shape[0] < 1 or item.shape[-1] != 3
-                    or item.device.type != "cpu"):
-                raise ValueError("encode_clips expects host uint8 clips [T, H, W, 3] with T >= 1; "
-                                 f"got {item.dtype} {tuple(item.shape)} on {item.device}")
+            item = _host_frames(item, "encode_clips", 1)
             training_geometry(item.shape[1], item.shape[2], size, resize)   # refuses a crop torchvision would pad
             yield item
 
-    # As in _reconstruct, no device context is held across the yields: every allocation, stream and launch names the
-    # model's device, and the kernels run on that device's current stream.
-    dev = model.device
-    copy = torch.cuda.Stream(device=dev)
-    staging: Optional[torch.Tensor] = None   # pinned upload buffer (flat), refilled once its last upload has completed
-    staged = torch.cuda.Event()
-    downloads: deque = deque()               # (host moments [B, 2z, t', h', w'], event of their download), oldest first
-
-    def results():
-        host, done = downloads.popleft()
-        done.synchronize()
-        return list(host.unbind(0))
-
+    # As in _reconstruct, no device context is held across the yields.  The `del`s free a clip's source frames once its
+    # slot is written and the batch's input once it is encoded, so device memory stays one batch deep.
+    io = _HostTransfers(model.device)
     for batch in clip_batches(checked(clips), batch_size):
-        compute = torch.cuda.current_stream(dev)
-        x = torch.empty((len(batch), 3, batch[0].shape[0], *size), dtype=model.dtype, device=dev)
+        x = torch.empty((len(batch), 3, batch[0].shape[0], *size), dtype=model.dtype, device=model.device)
         for i, clip in enumerate(batch):
-            # host -> pinned staging -> device on the copy stream; the compute stream waits for that upload only
-            staged.synchronize()
-            if staging is None or staging.numel() < clip.numel():
-                staging = torch.empty(clip.numel(), dtype=torch.uint8, pin_memory=True)
-            pinned = staging[:clip.numel()].view(clip.shape)
-            pinned.copy_(clip)
-            with torch.cuda.stream(copy):
-                src = torch.empty(clip.shape, dtype=torch.uint8, device=dev)
-                src.copy_(pinned, non_blocking=True)
-                staged.record(copy)
-            compute.wait_event(staged)
-            src.record_stream(compute)
+            src = io.upload(clip)
             frames_to_training_input(src, size, resize, model.dtype, out=x[i:i + 1])
             del src
         moments = model.encode(x).latent_dist.parameters
         del x
-        host = _pinned(moments.shape, moments)
-        copy.wait_stream(compute)
-        with torch.cuda.stream(copy):
-            host.copy_(moments, non_blocking=True)
-            done = torch.cuda.Event()
-            done.record(copy)
-        moments.record_stream(copy)
+        io.download(moments)
         del moments
-        downloads.append((host, done))
         # one-batch lag: a batch's moments go to the caller only once the next batch is enqueued behind it
-        while len(downloads) > 1:
-            yield from results()
-    while downloads:
-        yield from results()
+        while len(io) > 1:
+            yield from io.take()[0].unbind(0)
+    while io:
+        yield from io.take()[0].unbind(0)

@@ -28,15 +28,15 @@ def _check_frames(frames_u8: torch.Tensor, who: str) -> torch.Tensor:
     return frames_u8.contiguous()
 
 
+@L._on_tensor_device
 def resize_frames(frames_u8: torch.Tensor, size) -> torch.Tensor:
     """`transforms.Resize(size=(h, w))` of the script on the GPU: uint8 [T, H, W, 3] -> uint8 [T, h, w, 3]."""
     frames_u8 = _check_frames(frames_u8, "resize_frames")
     T, H, W, _ = frames_u8.shape
     oh, ow = int(size[0]), int(size[1])
     out = torch.empty((T, oh, ow, 3), dtype=torch.uint8, device=frames_u8.device)
-    with torch.cuda.device(frames_u8.device):
-        L.check(L.load().cvvae_video_resize_u8(frames_u8.data_ptr(), out.data_ptr(), None, T, H, W, oh, ow, L.F16,
-                                               torch.cuda.current_stream(out.device).cuda_stream), "cvvae_video_resize_u8")
+    L.check(L.load().cvvae_video_resize_u8(frames_u8.data_ptr(), out.data_ptr(), None, T, H, W, oh, ow, L.F16, L._stream(out)),
+            "cvvae_video_resize_u8")
     return out
 
 
@@ -52,6 +52,7 @@ def frames_to_input_and_u8(frames_u8: torch.Tensor, dtype: torch.dtype = torch.f
     return _to_input(frames_u8, dtype, size, True)
 
 
+@L._on_tensor_device
 def _to_input(frames_u8: torch.Tensor, dtype: torch.dtype, size, want_u8: bool):
     frames_u8 = _check_frames(frames_u8, "frames_to_input")
     T, H, W, _ = frames_u8.shape
@@ -59,14 +60,12 @@ def _to_input(frames_u8: torch.Tensor, dtype: torch.dtype, size, want_u8: bool):
         oh, ow = int(size[0]), int(size[1])
         out = torch.empty((1, 3, T, oh, ow), dtype=dtype, device=frames_u8.device)
         u8 = torch.empty((T, oh, ow, 3), dtype=torch.uint8, device=frames_u8.device) if want_u8 else None
-        with torch.cuda.device(frames_u8.device):
-            L.check(L.load().cvvae_video_resize_u8(frames_u8.data_ptr(), u8.data_ptr() if want_u8 else None, out.data_ptr(),
-                                                   T, H, W, oh, ow, dtype_code(dtype),
-                                                   torch.cuda.current_stream(out.device).cuda_stream), "cvvae_video_resize_u8")
+        L.check(L.load().cvvae_video_resize_u8(frames_u8.data_ptr(), u8.data_ptr() if want_u8 else None, out.data_ptr(),
+                                               T, H, W, oh, ow, dtype_code(dtype), L._stream(out)), "cvvae_video_resize_u8")
         return out, u8
     out = torch.empty((1, 3, T, H, W), dtype=dtype, device=frames_u8.device)
-    L.check(L.load().cvvae_video_u8_to_f16(frames_u8.data_ptr(), out.data_ptr(), T, H, W, dtype_code(dtype),
-                                           torch.cuda.current_stream(out.device).cuda_stream), "cvvae_video_u8_to_f16")
+    L.check(L.load().cvvae_video_u8_to_f16(frames_u8.data_ptr(), out.data_ptr(), T, H, W, dtype_code(dtype), L._stream(out)),
+            "cvvae_video_u8_to_f16")
     return out, frames_u8
 
 
@@ -116,6 +115,7 @@ def training_geometry(H: int, W: int, size, resize: str = "cover") -> tuple:
     return RH, RW, int(round((RH - h) / 2.0)), int(round((RW - w) / 2.0))
 
 
+@L._on_tensor_device
 def frames_to_training_input(frames_u8: torch.Tensor, size, resize: str = "cover", dtype: torch.dtype = torch.float16,
                              out: torch.Tensor = None) -> torch.Tensor:
     """The reference's training pre-processing on the GPU: uint8 [T, H, W, 3] -> [1, 3, T, h, w], (h, w) = size.
@@ -136,13 +136,12 @@ def frames_to_training_input(frames_u8: torch.Tensor, size, resize: str = "cover
           or not out.is_contiguous()):
         raise ValueError(f"frames_to_training_input: out must be a contiguous {dtype} tensor [1, 3, {T}, {h}, {w}] on "
                          f"{frames_u8.device}; got {out.dtype} {tuple(out.shape)} on {out.device}")
-    with torch.cuda.device(frames_u8.device):
-        L.check(L.load().cvvae_video_train_input(frames_u8.data_ptr(), out.data_ptr(), T, H, W, RH, RW, top, left, h, w,
-                                                 dtype_code(dtype), torch.cuda.current_stream(out.device).cuda_stream),
-                "cvvae_video_train_input")
+    L.check(L.load().cvvae_video_train_input(frames_u8.data_ptr(), out.data_ptr(), T, H, W, RH, RW, top, left, h, w,
+                                             dtype_code(dtype), L._stream(out)), "cvvae_video_train_input")
     return out
 
 
+@L._on_tensor_device
 def output_to_frames(x: torch.Tensor) -> torch.Tensor:
     """[1, 3, T, H, W] reconstruction -> uint8 [T, H, W, 3] (clamped to [-1, 1], scaled to 0..255)."""
     if x.dim() != 5 or x.shape[0] != 1 or x.shape[1] != 3 or not x.is_cuda:
@@ -150,6 +149,6 @@ def output_to_frames(x: torch.Tensor) -> torch.Tensor:
     x = x.contiguous()
     _, _, T, H, W = x.shape
     out = torch.empty((T, H, W, 3), dtype=torch.uint8, device=x.device)
-    L.check(L.load().cvvae_video_f16_to_u8(x.data_ptr(), out.data_ptr(), T, H, W, dtype_code(x.dtype),
-                                           torch.cuda.current_stream(x.device).cuda_stream), "cvvae_video_f16_to_u8")
+    L.check(L.load().cvvae_video_f16_to_u8(x.data_ptr(), out.data_ptr(), T, H, W, dtype_code(x.dtype), L._stream(x)),
+            "cvvae_video_f16_to_u8")
     return out

@@ -1,6 +1,7 @@
 """StreamEncoder / StreamDecoder / reconstruct_frames on the H100: bit-exact against the whole-clip calls in every dtype,
 eager and with CUDA graphs, at the fixtures' sizes and at 49x576x1024; device memory flat in the clip length; the
-host-to-host reconstruction chain equal to the reference script's whole-clip chain."""
+host-to-host reconstruction chain equal to the reference script's whole-clip chain, also for a model on a device other
+than the current one."""
 import json
 import os
 import random
@@ -166,6 +167,29 @@ def test_reconstruct_frames_bit_exact(name, T, size):
     assert all(p.dtype == torch.uint8 and p.device.type == "cpu" for p in pieces)
     got = torch.cat(pieces, dim=0)
     assert got.shape == want.shape and torch.equal(got, want)
+
+
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs")
+def test_model_on_another_device_than_the_current_one():
+    """A model on cuda:1 while cuda:0 is current: the host-facing streams and the pixel conversions launch on the model's
+    device, and give the bits the same calls give on cuda:0."""
+    from cvvae_b200 import encode_clips, evaluate_frames, reconstruct_frames
+    from cvvae_b200.video_io import frames_to_input, output_to_frames
+    frames = torch.randint(0, 256, (9, 64, 80, 3), generator=torch.Generator().manual_seed(9), dtype=torch.uint8)
+    items = [frames[:4], frames[4:].numpy()]
+
+    def calls(dev):
+        m = _build("sd21", 32, {}, torch.float16).to(dev)
+        x = frames_to_input(frames.to(dev), dtype=m.dtype)
+        scored = list(evaluate_frames(m, items))
+        return [x.cpu(), output_to_frames(x).cpu(), torch.cat(list(reconstruct_frames(m, items))),
+                *(torch.cat(parts) for parts in zip(*scored)), *encode_clips(m, [frames[:5], frames.numpy()], (64, 80))]
+
+    want = calls("cuda:0")
+    with torch.cuda.device(0):
+        got = calls("cuda:1")
+    assert len(got) == len(want) == 8
+    assert all(torch.equal(a, b) for a, b in zip(got, want))
 
 
 def test_reconstruct_frames_sample_posterior_is_seeded():

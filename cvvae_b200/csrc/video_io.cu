@@ -1,6 +1,7 @@
 // Pixel pre/post-processing either side of encode()/decode(), fused into one pass each (SURVEY.md section 8f row 3):
 //   uint8 [T,H,W,3] frames  ->  16-bit [1,3,T,H,W] in [-1,1]   (cvvae_inference_video.py:30-38: `.half() / 127.5 - 1.0`)
 //   16-bit [1,3,T,H,W]      ->  uint8 [T,H,W,3]                (cvvae_inference_video.py:47-50: clamp, +1, *127.5, uint8)
+//   [B,3,T,H,W] (F16 / BF16 / F32) -> uint8 [B,T,H,W,3]         (the same expression over a batch of decoded clips)
 // Bit-exact with the reference expressions: every intermediate is rounded to the 16-bit type exactly where PyTorch
 // rounds it (each elementwise op reads/writes the tensor dtype, arithmetic in fp32).
 #include "common.cuh"
@@ -22,21 +23,40 @@ __global__ void __launch_bounds__(256) u8_to_f16_kernel(const uint8_t* __restric
   }
 }
 
+// [B,3,T,H,W] -> uint8 [B,T,H,W,3], sample b on blockIdx.y (and every gridDim.y-th sample after it), pixels of a sample on
+// the x grid, so no thread divides an index.  16-bit types: each intermediate is rounded to the type; F32 (from_f is the
+// identity): two single fp32 roundings, as PyTorch evaluates the expression on a float32 tensor.
 template <int DT>
 __global__ void __launch_bounds__(256) f16_to_u8_kernel(const typename Elem<DT>::T* __restrict__ in, uint8_t* __restrict__ out,
-                                                        long long thw) {
+                                                        long long thw, int B) {
   using E = Elem<DT>;
-  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < thw;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+  for (int b = blockIdx.y; b < B; b += gridDim.y) {
+    const typename E::T* src = in + 3ll * b * thw;
+    uint8_t* dst = out + 3ll * b * thw;
+    for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < thw;
+         i += static_cast<long long>(gridDim.x) * blockDim.x) {
 #pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      float v = E::to_f(in[c * thw + i]);
-      v = fminf(fmaxf(v, -1.0f), 1.0f);                 // torch.clamp(x, -1, 1)   (NaN propagates like torch: stays NaN)
-      const typename E::T a = E::from_f(v + 1.0f);      // + 1.0
-      const typename E::T m = E::from_f(E::to_f(a) * 127.5f);  // * 127.5
-      out[i * 3 + c] = static_cast<uint8_t>(static_cast<int>(E::to_f(m)));   // .to(uint8): truncation
+      for (int c = 0; c < 3; ++c) {
+        float v = E::to_f(src[c * thw + i]);
+        v = fminf(fmaxf(v, -1.0f), 1.0f);                         // torch.clamp(x, -1, 1)   (NaN: undefined below)
+        const typename E::T a = E::from_f(__fadd_rn(v, 1.0f));            // + 1.0
+        const typename E::T m = E::from_f(__fmul_rn(E::to_f(a), 127.5f));  // * 127.5
+        dst[i * 3 + c] = static_cast<uint8_t>(static_cast<int>(E::to_f(m)));   // .to(uint8): truncation
+      }
     }
   }
+}
+
+// The one launch of f16_to_u8_kernel for B samples of thw pixels each (arguments checked by the caller).
+template <int DT>
+void launch_output_u8(const void* in, uint8_t* out, int B, long long thw, cudaStream_t stream) {
+  const long long target = 16ll * num_sms();
+  const long long bx = thw / 256 + 1 < target ? thw / 256 + 1 : target;
+  const int by = B < 65535 ? B : 65535;
+  // B == 1: the grid of the single-sample entry point; more samples split the same number of CTAs between them
+  const long long per = bx * by > target ? (target / by > 0 ? target / by : 1) : bx;
+  f16_to_u8_kernel<DT><<<dim3(static_cast<unsigned>(per), static_cast<unsigned>(by)), 256, 0, stream>>>(
+      reinterpret_cast<const typename Elem<DT>::T*>(in), out, thw, B);
 }
 
 // Antialiased bilinear resize of uint8 frames [T,H,W,3] -> [T,OH,OW,3] (torchvision `transforms.Resize(size)` on a uint8
@@ -217,11 +237,22 @@ extern "C" int cvvae_video_f16_to_u8(const void* in_cthw, uint8_t* thwc, int32_t
                                      void* stream) {
   CVVAE_CHECK_ARG(thwc && in_cthw && T > 0 && H > 0 && W > 0, "cvvae_video_f16_to_u8: bad argument");
   const long long thw = 1ll * T * H * W;
-  const unsigned blocks = static_cast<unsigned>(thw / 256 + 1 < 16ll * num_sms() ? thw / 256 + 1 : 16ll * num_sms());
-  CVVAE_DISPATCH_DTYPE16(dtype, "video_io", {
-    f16_to_u8_kernel<DT><<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        reinterpret_cast<const typename Elem<DT>::T*>(in_cthw), thwc, thw);
-  });
+  CVVAE_DISPATCH_DTYPE16(dtype, "video_io", { launch_output_u8<DT>(in_cthw, thwc, 1, thw, static_cast<cudaStream_t>(stream)); });
+  CVVAE_LAUNCH_CHECK();
+  return CVVAE_OK;
+}
+
+extern "C" int cvvae_video_output_u8(const void* in_bcthw, uint8_t* out_bthwc, int32_t B, int32_t T, int32_t H, int32_t W,
+                                     int32_t dtype, void* stream) {
+  CVVAE_CHECK_ARG(in_bcthw && out_bthwc && B > 0 && T > 0 && H > 0 && W > 0,
+                  "cvvae_video_output_u8: bad argument (in=%p out=%p B=%d T=%d H=%d W=%d)", in_bcthw,
+                  static_cast<const void*>(out_bthwc), B, T, H, W);
+  long long n = 3ll * B;   // elements of either tensor: every index the kernel forms is below it
+  const bool overflow = __builtin_mul_overflow(n, 1ll * T, &n) || __builtin_mul_overflow(n, 1ll * H, &n) ||
+                        __builtin_mul_overflow(n, 1ll * W, &n);
+  CVVAE_CHECK_ARG(!overflow, "cvvae_video_output_u8: 3 x %d x %d x %d x %d elements overflow a 64-bit index", B, T, H, W);
+  const long long thw = 1ll * T * H * W;
+  CVVAE_DISPATCH_DTYPE(dtype, { launch_output_u8<DT>(in_bcthw, out_bthwc, B, thw, static_cast<cudaStream_t>(stream)); });
   CVVAE_LAUNCH_CHECK();
   return CVVAE_OK;
 }

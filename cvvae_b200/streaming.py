@@ -15,7 +15,8 @@ reconstructed frame scored (PSNR, SSIM) on the device against the input frame th
 
 ``encode_clips`` turns a dataset of clips into latents: each clip goes through the reference's training pre-processing
 (``video_io.frames_to_training_input``) straight into its slot of a batch, and batches of clips with equal length run
-through one ``model.encode`` call each.
+through one ``model.encode`` call each.  ``decode_clips`` is the way back: batches of clip latents of equal shape run
+through one ``model.tiled_decode`` call and one pixel conversion each, and come back as uint8 videos.
 """
 from __future__ import annotations
 
@@ -160,16 +161,17 @@ class _HostTransfers:
         """Downloads queued and not yet taken."""
         return len(self._downloads)
 
-    def upload(self, host_u8: torch.Tensor) -> torch.Tensor:
-        """host -> pinned staging -> device on the copy stream; the compute stream waits for that upload only."""
-        n = host_u8.numel()
+    def upload(self, host: torch.Tensor) -> torch.Tensor:
+        """host -> pinned staging -> device on the copy stream; the compute stream waits for that upload only.  The
+        staging buffer holds bytes: it is viewed as `host`'s dtype, whatever that is."""
+        n = host.numel() * host.element_size()
         self._staged.synchronize()
         if self._staging is None or self._staging.numel() < n:
             self._staging = _pinned(n, torch.uint8)
-        pinned = self._staging[:n].view(host_u8.shape)
-        pinned.copy_(host_u8)
+        pinned = self._staging[:n].view(host.dtype).view(host.shape)
+        pinned.copy_(host)
         with torch.cuda.stream(self._copy):
-            out = torch.empty(host_u8.shape, dtype=torch.uint8, device=self._dev)
+            out = torch.empty(host.shape, dtype=host.dtype, device=self._dev)
             out.copy_(pinned, non_blocking=True)
             self._staged.record(self._copy)
         compute = torch.cuda.current_stream(self._dev)
@@ -345,9 +347,10 @@ def _reconstruct(model, enc: StreamEncoder, dec: StreamDecoder, frames: Iterator
 
 
 def clip_batches(clips: Iterable, batch_size: int, length=len) -> Iterator[list]:
-    """The batching schedule of ``encode_clips``: consecutive clips of equal ``length(clip)`` in batches of at most
-    `batch_size`, in input order.  A batch closes as soon as it is full, when a clip of another length arrives, or at the
-    end of the input; it is yielded then, before the next clip is read."""
+    """The batching schedule of ``encode_clips`` and ``decode_clips``: consecutive clips of equal ``length(clip)`` (for
+    ``decode_clips``, a clip's latent shape) in batches of at most `batch_size`, in input order.  A batch closes as soon
+    as it is full, when a clip of another length arrives, or at the end of the input; it is yielded then, before the next
+    clip is read."""
     batch: list = []
     for clip in clips:
         if batch and length(clip) != length(batch[0]):
@@ -421,6 +424,82 @@ def _encode_clips(model, clips: Iterator, size: tuple, resize: str, batch_size: 
         io.download(moments)
         del moments
         # one-batch lag: a batch's moments go to the caller only once the next batch is enqueued behind it
+        while len(io) > 1:
+            yield from io.take()[0].unbind(0)
+    while io:
+        yield from io.take()[0].unbind(0)
+
+
+def decode_clips(model, latents: Iterable, batch_size: int = 8) -> Iterator[torch.Tensor]:
+    """Decode a dataset of clip latents to uint8 videos, batched on the GPU: the mirror of ``encode_clips``.
+
+    `latents` is an iterable of one clip's latents each, ``[z, t', h, w]`` with t' >= 1, in the model's dtype: numpy
+    arrays, CPU tensors or tensors on the model's device (a posterior's ``mode()[0]``, or a diffusion model's sample,
+    scaled as ``model.decode`` expects).  Yields, for each clip in input order, a host uint8 ``[T, H, W, 3]`` tensor,
+    T = ``model._engine().decoded_frames(t')``, equal bit for bit to::
+
+        x = model.tiled_decode(z[None].to(model.device))     # what model.decode(z[None]).sample runs on 5-D latents
+        output_to_frames(x)                                   # float16 / bfloat16 models
+        ((x.clamp(-1, 1) + 1.0) * 127.5).to(torch.uint8)[0].permute(1, 2, 3, 0)   # float32 models, evaluated by torch
+
+    Consecutive clips of equal ``(t', h, w)`` are stacked into one ``[B, z, t', h, w]`` batch (B <= `batch_size`, see
+    ``clip_batches``), which runs through one ``model.tiled_decode`` call, with the model's chunking, tiling and CUDA
+    graphs, and one ``video_io.batch_to_frames`` launch.  Batching changes no clip's frames: nothing in the engine mixes
+    samples.
+
+    Uploads and downloads run on a side stream, overlapped with the kernels on the device's current stream, and a batch's
+    frames are yielded once the next batch has been enqueued.  Device memory holds one batch's latents, activations,
+    decoded pixels and uint8 frames plus the download in flight, however many clips there are.  Yielded tensors are the
+    caller's: later yields never overwrite them.
+
+    Raises ValueError at the call for a model that is not on CUDA or a `batch_size` that is not an int >= 1, and when an
+    item arrives that is not ``[z, t', h, w]`` with t', h, w >= 1, or whose dtype or device is not the model's (nothing is
+    cast).
+    """
+    if model.device.type != "cuda":
+        raise ValueError("decode_clips: the model must be on a CUDA device")
+    if isinstance(batch_size, bool) or not isinstance(batch_size, int) or batch_size < 1:
+        raise ValueError(f"decode_clips: batch_size must be an int >= 1; got {batch_size!r}")
+    return _decode_clips(model, iter(latents), batch_size)
+
+
+def _clip_latents(item, z_channels: int, dtype: torch.dtype, device: torch.device) -> torch.Tensor:
+    """One clip's latents (numpy array or tensor) as a host or `device` tensor [z, t', h, w]; ValueError otherwise."""
+    item = torch.as_tensor(item)
+    if item.dim() != 4 or item.shape[0] != z_channels or min(item.shape[1:]) < 1:
+        raise ValueError(f"decode_clips expects latents [{z_channels}, t', h, w] with t', h, w >= 1; got {tuple(item.shape)}")
+    if item.dtype != dtype:
+        raise ValueError(f"decode_clips: latents are {item.dtype}, the model is {dtype}; cast them first")
+    if item.device.type != "cpu" and item.device != device:
+        raise ValueError(f"decode_clips: latents on {item.device} for a model on {device}; pass host tensors or tensors "
+                         "on the model's device")
+    return item
+
+
+def _decode_clips(model, latents: Iterator, batch_size: int) -> Iterator[torch.Tensor]:
+    from .video_io import batch_to_frames
+
+    dev, dtype, z_channels = model.device, model.dtype, model.net.z_channels
+    checked = (_clip_latents(item, z_channels, dtype, dev) for item in latents)
+    # As in _encode_clips, no device context is held across the yields, and the `del`s keep device memory one batch deep.
+    io = _HostTransfers(dev)
+    for batch in clip_batches(checked, batch_size, length=lambda z: tuple(z.shape)):
+        z = torch.empty((len(batch), *batch[0].shape), dtype=dtype, device=dev)
+        for i, item in enumerate(batch):
+            if item.device.type == "cpu":
+                src = io.upload(item)
+                z[i].copy_(src)
+                del src
+            else:
+                z[i].copy_(item)
+        model._maybe_offload_hook()
+        x = model.tiled_decode(z)
+        del z
+        frames = batch_to_frames(x)
+        del x
+        io.download(frames)
+        del frames
+        # one-batch lag: a batch's frames go to the caller only once the next batch is enqueued behind it
         while len(io) > 1:
             yield from io.take()[0].unbind(0)
     while io:

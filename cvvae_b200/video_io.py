@@ -6,7 +6,8 @@
 (cvvae_inference_video.py:30-38 and :47-50).  Bit-exact with those expressions.  The script's spatial resize
 (`transforms.Resize(size=(height, width))` on the uint8 frames, :15-17,28) is available on the GPU as well:
 `resize_frames(frames, size)` / `frames_to_input(frames, size=...)` (antialiased bilinear, within 1 LSB of torchvision's
-fixed-point uint8 path, which differs from exact arithmetic on < 1 % of the pixels).
+fixed-point uint8 path, which differs from exact arithmetic on < 1 % of the pixels).  `batch_to_frames(x)` is the output
+conversion over a batch [B, 3, T, H, W] in float16, bfloat16 or float32, one launch for all clips.
 
 The reference's *training* data path prepares frames differently (lvdm/data/decoder.py:99-109, transform.py): float
 first, then CoverResize / Resize(short side) and CenterCrop, then `(x / 255 - 0.5) * 2`, never rounded to uint8.
@@ -151,4 +152,27 @@ def output_to_frames(x: torch.Tensor) -> torch.Tensor:
     out = torch.empty((T, H, W, 3), dtype=torch.uint8, device=x.device)
     L.check(L.load().cvvae_video_f16_to_u8(x.data_ptr(), out.data_ptr(), T, H, W, dtype_code(x.dtype), L._stream(x)),
             "cvvae_video_f16_to_u8")
+    return out
+
+
+@L._on_tensor_device
+def batch_to_frames(x: torch.Tensor, out: torch.Tensor = None) -> torch.Tensor:
+    """A batch of reconstructions [B, 3, T, H, W] (float16, bfloat16 or float32) -> uint8 [B, T, H, W, 3] in one launch.
+
+    Every element is ``((clamp(x, -1, 1) + 1.0) * 127.5).to(uint8)`` as PyTorch evaluates it in x's dtype, so for 16-bit
+    types slot b equals ``output_to_frames(x[b:b + 1])``.  `out`, if given, is a contiguous uint8 [B, T, H, W, 3] tensor on
+    x's device, written in place and returned."""
+    if x.dim() != 5 or x.shape[1] != 3 or not x.is_cuda or x.dtype not in (torch.float16, torch.bfloat16, torch.float32):
+        raise ValueError("batch_to_frames expects a CUDA float16, bfloat16 or float32 tensor [B, 3, T, H, W]; got "
+                         f"{x.dtype} {tuple(x.shape)} on {x.device}")
+    x = x.contiguous()
+    B, _, T, H, W = x.shape
+    if out is None:
+        out = torch.empty((B, T, H, W, 3), dtype=torch.uint8, device=x.device)
+    elif (tuple(out.shape) != (B, T, H, W, 3) or out.dtype != torch.uint8 or out.device != x.device
+          or not out.is_contiguous()):
+        raise ValueError(f"batch_to_frames: out must be a contiguous uint8 tensor [{B}, {T}, {H}, {W}, 3] on {x.device}; "
+                         f"got {out.dtype} {tuple(out.shape)} on {out.device}")
+    L.check(L.load().cvvae_video_output_u8(x.data_ptr(), out.data_ptr(), B, T, H, W, dtype_code(x.dtype), L._stream(x)),
+            "cvvae_video_output_u8")
     return out

@@ -21,7 +21,8 @@
  *     consumers are tensor-core products (packed weights, GroupNorm / LayerNorm / softmax outputs, pack_taps_hw and the
  *     channels-first -> channels-last copy of a network input) are stored rounded to the nearest TF32 value; every other output
  *     (convolution outputs: residual stream, q / k / v, attention output) is full fp32.  The video_io entry points of the
- *     inference script and cvvae_conv3d_stacked are 16-bit only and reject CVVAE_F32; cvvae_video_train_input takes all three.
+ *     inference script and cvvae_conv3d_stacked are 16-bit only and reject CVVAE_F32; cvvae_video_train_input and
+ *     cvvae_video_output_u8 take all three.
  */
 #ifndef CVVAE_B200_H_
 #define CVVAE_B200_H_
@@ -189,6 +190,13 @@ int cvvae_blend(const cvvae_tensor5* a, const cvvae_tensor5* b, int32_t overlap,
  * Both tensors are contiguous device buffers. */
 int cvvae_video_u8_to_f16(const uint8_t* thwc, void* out_cthw, int32_t T, int32_t H, int32_t W, int32_t dtype, void* stream);
 int cvvae_video_f16_to_u8(const void* in_cthw, uint8_t* thwc, int32_t T, int32_t H, int32_t W, int32_t dtype, void* stream);
+/* f16_to_u8 over a batch, in any activation dtype: [B,3,T,H,W] (CVVAE_F16, CVVAE_BF16 or CVVAE_F32) -> uint8 [B,T,H,W,3],
+ * both contiguous on the device, every element ((clamp(x,-1,1) + 1.0) * 127.5).to(uint8) as PyTorch evaluates it in the
+ * tensor's dtype: 16-bit types round every intermediate to the type, CVVAE_F32 makes two single fp32 roundings.  NaN
+ * inputs give an unspecified byte (the cast is undefined in PyTorch too).  A null pointer, B or a size < 1, an element
+ * count 3*B*T*H*W beyond int64 or an unknown dtype is CVVAE_E_ARG before any launch.  One kernel launch. */
+int cvvae_video_output_u8(const void* in_bcthw, uint8_t* out_bthwc, int32_t B, int32_t T, int32_t H, int32_t W,
+                          int32_t dtype, void* stream);
 /* The script's `transforms.Resize(size=(height, width))` on the uint8 frames (cvvae_inference_video.py:15-17,28), on the GPU:
  * antialiased bilinear (triangle filter, support scaled by the down-scale factor, round half up), uint8 [T,H,W,3] ->
  * out_thwc uint8 [T,OH,OW,3] and/or out_cthw 16-bit [3,T,OH,OW] = resized.half() / 127.5 - 1.0 (either may be NULL).

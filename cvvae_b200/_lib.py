@@ -69,6 +69,9 @@ _SIGNATURES = {
     "cvvae_video_train_input": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                           C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     "cvvae_frame_metrics": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "cvvae_frame_ms_ssim": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                      C.c_void_p]),
+    "cvvae_ms_ssim_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32]),
     "cvvae_conv_tc_set_trace": (C.c_int, [C.c_void_p, C.c_int32]),
     "cvvae_conv_tc_plan": (C.c_int, [C.POINTER(ConvDesc), C.POINTER(C.c_int32), C.c_int32]),
     "cvvae_last_error": (C.c_char_p, []),

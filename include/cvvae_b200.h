@@ -228,6 +228,23 @@ int cvvae_video_train_input(const uint8_t* thwc, void* out_cthw, int32_t T, int3
  * T >= 0 (T == 0 launches nothing), H, W >= 11 and 3*H*W < 2^31, else CVVAE_E_ARG.  One kernel launch. */
 int cvvae_frame_metrics(const uint8_t* a_thwc, const uint8_t* b_thwc, int32_t T, int32_t H, int32_t W, int64_t* acc,
                         void* stream);
+/* Multi-scale SSIM (Wang, Simoncelli and Bovik 2003) of the same two videos, as per-level sums; the caller combines them.
+ * Level 0 is the frames; level j+1 is the 2x2 average pool of level j, an odd extent zero-padded in front (output i of an
+ * axis of odd length covers inputs 2i-1 and 2i, input -1 being 0; the divisor stays 4).  At each level j = 0..4, per
+ * colour channel c and over the positions whose 11x11 window lies inside the level-j image, with the SSIM conventions
+ * above (data range 255 at every level):
+ *   acc: int64 [T][5][3][2], overwritten:  acc[t][j][c][0] = sum of llrint(cs * 2^32),  cs = (2 s_ab + C2) / (s_a^2 + s_b^2 + C2)
+ *                                          acc[t][j][c][1] = sum of llrint(ssim * 2^32)
+ * The level-j image is ceil(H / 2^j) x ceil(W / 2^j).  MS-SSIM(c) = prod_{j<4} max(cs_j, 0)^w_j * max(ssim_4, 0)^w_4 with
+ * the means cs_j, ssim_j over the positions and w = (0.0448, 0.2856, 0.3001, 0.2363, 0.1333); the frame's score is the
+ * mean over c.  Levels 1-4 are kept as exact integer sums (uint16) in `workspace`: device memory of at least
+ * cvvae_ms_ssim_workspace_bytes(T, H, W) bytes, 16-byte aligned.  Identical frames give exactly 2^32 per position.
+ * T >= 0 (T == 0 launches nothing), H, W >= 161 and 3*H*W < 2^31, else CVVAE_E_ARG.  Nine kernel launches: the five
+ * levels' scores and four pooling steps. */
+int cvvae_frame_ms_ssim(const uint8_t* a_thwc, const uint8_t* b_thwc, int32_t T, int32_t H, int32_t W, void* workspace,
+                        int64_t* acc, void* stream);
+/* Bytes of the workspace cvvae_frame_ms_ssim needs for T frames of H x W px (T >= 0, H, W >= 1; else CVVAE_E_ARG). */
+int64_t cvvae_ms_ssim_workspace_bytes(int32_t T, int32_t H, int32_t W);
 
 /* Diagnostics */
 /* Per-CTA phase timestamps of the next conv_tc launches: device buffer of n_ctas x 8 uint64 (globaltimer ns:

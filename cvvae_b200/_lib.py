@@ -15,6 +15,7 @@ from ._build import LIBPATH
 F16, BF16, F32 = 0, 1, 2
 PAD_ZERO, PAD_REPLICATE = 0, 1
 CONV_BIAS_ALONG_M, CONV_FORCE_DIRECT, CONV_OUT_F32, CONV_W_PER_BATCH, CONV_X_SHARED = 1, 2, 4, 8, 16
+CONV_RELU, CONV_TF32_OUT = 32, 64
 ABI_VERSION = 3
 
 
@@ -72,6 +73,9 @@ _SIGNATURES = {
     "cvvae_frame_ms_ssim": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                       C.c_void_p]),
     "cvvae_ms_ssim_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32]),
+    "cvvae_lpips_input": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "cvvae_lpips_tap": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                  C.c_void_p]),
     "cvvae_conv_tc_set_trace": (C.c_int, [C.c_void_p, C.c_int32]),
     "cvvae_conv_tc_plan": (C.c_int, [C.POINTER(ConvDesc), C.POINTER(C.c_int32), C.c_int32]),
     "cvvae_last_error": (C.c_char_p, []),

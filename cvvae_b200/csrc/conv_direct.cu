@@ -154,6 +154,7 @@ __global__ void pack_weight_kernel(const typename Elem<DT>::T* __restrict__ src,
 }
 
 bool conv_tc_eligible(const cvvae_conv_desc* d, const char** why);
+int conv_relu_check(const cvvae_conv_desc* d);
 int conv_tc_launch(const cvvae_conv_desc* d, cudaStream_t stream);
 int gn_stats_run(const cvvae_tensor5* x, int32_t groups, int32_t per_frame, int64_t* stats, int32_t dtype,
                  cudaStream_t stream, bool zero_first);
@@ -162,6 +163,8 @@ int gn_stats_run(const cvvae_tensor5* x, int32_t groups, int32_t per_frame, int6
 
 extern "C" int cvvae_conv3d_direct(const cvvae_conv_desc* d, void* stream) {
   CVVAE_CHECK_ARG(d && cvvae::tensor_ok(&d->x) && cvvae::tensor_ok(&d->y) && d->w, "cvvae_conv3d_direct: null argument");
+  CVVAE_CHECK_ARG(!(d->flags & (CVVAE_CONV_RELU | CVVAE_CONV_TF32_OUT)),
+                  "cvvae_conv3d_direct: CVVAE_CONV_RELU / CVVAE_CONV_TF32_OUT are tensor-core epilogue features");
   return cvvae::conv_direct_launch(d, static_cast<cudaStream_t>(stream));
 }
 
@@ -169,6 +172,11 @@ extern "C" int cvvae_conv3d(const cvvae_conv_desc* d, void* stream_) {
   CVVAE_CHECK_ARG(d && cvvae::tensor_ok(&d->x) && cvvae::tensor_ok(&d->y) && d->w, "cvvae_conv3d: null argument");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const bool tc = !(d->flags & CVVAE_CONV_FORCE_DIRECT) && cvvae::conv_tc_eligible(d, nullptr);
+  if (d->flags & (CVVAE_CONV_RELU | CVVAE_CONV_TF32_OUT)) {
+    const int rc = cvvae::conv_relu_check(d);
+    if (rc != CVVAE_OK) return rc;
+    CVVAE_CHECK_ARG(tc, "cvvae_conv3d: CVVAE_CONV_RELU needs a descriptor the tensor-core path takes");
+  }
   if (!d->gn_stats) return tc ? cvvae::conv_tc_launch(d, stream) : cvvae::conv_direct_launch(d, stream);
   // consumer GroupNorm sums requested: fused in the tensor-core epilogue when that path can, otherwise one extra
   // statistics pass over y - either way `gn_stats` has y's sums added when the call returns

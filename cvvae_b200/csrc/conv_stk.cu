@@ -205,8 +205,9 @@ extern "C" int cvvae_conv3d_stacked(const cvvae_conv_desc* d, void* stream_) {
   CVVAE_CHECK_ARG(d->KH == 3 && d->KW == 3 && d->st == 1 && d->sh == 1 && d->sw == 1 && d->up_time != 2,
                   "cvvae_conv3d_stacked: needs a stride-1 (KT x) 3 x 3 convolution");
   CVVAE_CHECK_ARG(d->Cout >= 1 && d->Cout <= 4 && y.C == d->Cout, "cvvae_conv3d_stacked: Cout %d not in 1..4", d->Cout);
-  CVVAE_CHECK_ARG(!d->residual && !d->gn_stats && !(d->flags & (CVVAE_CONV_OUT_F32 | CVVAE_CONV_BIAS_ALONG_M)),
-                  "cvvae_conv3d_stacked: residual / statistics / fp32 output are not supported");
+  CVVAE_CHECK_ARG(!d->residual && !d->gn_stats && !(d->flags & (CVVAE_CONV_OUT_F32 | CVVAE_CONV_BIAS_ALONG_M | CVVAE_CONV_RELU |
+                                                                    CVVAE_CONV_TF32_OUT)),
+                  "cvvae_conv3d_stacked: residual / statistics / fp32 output / ReLU are not supported");
   CVVAE_CHECK_ARG(tma_view(x, 2) && reinterpret_cast<uintptr_t>(d->w) % 16 == 0 && x.C % 8 == 0,
                   "cvvae_conv3d_stacked: input must be a 16-byte aligned channels-last view");
   if (d->pad_hw != CVVAE_PAD_ZERO) {

@@ -64,6 +64,14 @@ static constexpr int kProducerRegs = 40, kMmaRegs = 232;   // 128 * 40 + 256 * 2
 static constexpr uint32_t kBarBytes = 2048;                // barriers + GroupNorm bins after the operand rings
 
 __device__ __forceinline__ void wait_bar(uint64_t* bar, uint32_t parity) { ptx::mbar_wait(bar, parity); }
+// max(v, 0) with -0 -> +0, which is what `clamp_min(0)` of the unfused output stores once a +0 is added
+__device__ __forceinline__ float relu_f(float v) { return v > 0.f ? v : 0.f; }
+// The ReLU epilogue's store: max(v, 0), rounded to the nearest TF32 value when the output's only consumers are tensor-core
+// products (CVVAE_CONV_TF32_OUT; the tensor cores would otherwise drop its low 13 bits, a truncation)
+__device__ __forceinline__ float relu_out(float v, int flags) {
+  v = relu_f(v);
+  return (flags & CVVAE_CONV_TF32_OUT) ? tf32_rn(v) : v;
+}
 
 struct TileCoord {
   int b, t, h0, w0, n0;
@@ -125,7 +133,10 @@ __device__ __forceinline__ void epi_piece(const ConvTcParams& p, const TileCoord
   }
 }
 
-template <int DT, int BN>
+// RELU: y = max(alpha * acc + bias, 0) in the register epilogue (CVVAE_CONV_RELU; fp32 storage only, without residual,
+// statistics or interleave, so only the register epilogue's loops carry it), stored rounded to TF32 with
+// CVVAE_CONV_TF32_OUT.
+template <int DT, int BN, bool RELU>
 __global__ void __launch_bounds__(kThreads, 1)
     conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                    const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
@@ -575,6 +586,10 @@ __global__ void __launch_bounds__(kThreads, 1)
             for (int rr = 0; rr < 2; ++rr) {
               float a0 = fmaf(acc[s][4 * j + 2 * rr], p.alpha, b0);
               float a1 = fmaf(acc[s][4 * j + 2 * rr + 1], p.alpha, b1);
+              if constexpr (RELU) {
+                a0 = relu_out(a0, p.flags);
+                a1 = relu_out(a1, p.flags);
+              }
               const long long off = roff[s][rr] + coff;
               if (p.residual) {
                 const float2 rf = E::to_f2(__ldg(reinterpret_cast<const typename E::P*>(reinterpret_cast<const T*>(p.residual) + off)));
@@ -620,6 +635,10 @@ __global__ void __launch_bounds__(kThreads, 1)
             const float bb0 = bias_m ? rbias[s][rr] : b0, bb1 = bias_m ? rbias[s][rr] : b1;
             float a0 = fmaf(acc[s][4 * j + 2 * rr], p.alpha, bb0);
             float a1 = fmaf(acc[s][4 * j + 2 * rr + 1], p.alpha, bb1);
+            if constexpr (RELU) {
+              a0 = relu_out(a0, p.flags);
+              a1 = relu_out(a1, p.flags);
+            }
             const long long off = roff[s][rr] + coff;
             if (out_f32) {
               // fp32 logits (S = q k^T): no residual, no interleave
@@ -722,16 +741,16 @@ void conv_tc_set_trace(unsigned long long* buf, int n) {
   g_trace_n = n;
 }
 
-template <int DT, int BN>
+template <int DT, int BN, bool RELU = false>
 static int launch_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmA2, const CUtensorMap& tmB2,
                      const CUtensorMap& tmY, const CUtensorMap& tmR, const ConvTcParams& p, unsigned grid, size_t smem,
                      cudaStream_t stream) {
   static PerDeviceOnce attr_set;   // the > 48 KB shared-memory opt-in is per device
   if (attr_set.need()) {
-    CVVAE_CUDA(cudaFuncSetAttribute(conv_tc_kernel<DT, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
+    CVVAE_CUDA(cudaFuncSetAttribute(conv_tc_kernel<DT, BN, RELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
     attr_set.mark();
   }
-  conv_tc_kernel<DT, BN><<<grid, kThreads, smem, stream>>>(tmA, tmB, tmA2, tmB2, tmY, tmR, p);
+  conv_tc_kernel<DT, BN, RELU><<<grid, kThreads, smem, stream>>>(tmA, tmB, tmA2, tmB2, tmY, tmR, p);
   return CVVAE_OK;
 }
 
@@ -871,7 +890,23 @@ static int conv_tc_plan(const cvvae_conv_desc* d, ConvTcParams& p, size_t& smem,
   return CVVAE_OK;
 }
 
+// CVVAE_CONV_RELU is a feature of the fp32 register epilogue alone: every combination it does not cover is refused here,
+// before anything is launched, by each entry point that takes a descriptor.
+int conv_relu_check(const cvvae_conv_desc* d) {
+  if (!(d->flags & (CVVAE_CONV_RELU | CVVAE_CONV_TF32_OUT))) return CVVAE_OK;
+  CVVAE_CHECK_ARG(d->flags & CVVAE_CONV_RELU, "conv: CVVAE_CONV_TF32_OUT is a store of the CVVAE_CONV_RELU epilogue");
+  CVVAE_CHECK_ARG(d->dtype == CVVAE_F32, "conv: CVVAE_CONV_RELU needs CVVAE_F32 activations, got dtype %d", (int)d->dtype);
+  CVVAE_CHECK_ARG(!d->residual && !d->w2 && !d->gn_stats && d->up_time != 2 &&
+                      !(d->flags & (CVVAE_CONV_OUT_F32 | CVVAE_CONV_W_PER_BATCH | CVVAE_CONV_X_SHARED | CVVAE_CONV_BIAS_ALONG_M |
+                                    CVVAE_CONV_FORCE_DIRECT)),
+                  "conv: CVVAE_CONV_RELU excludes a residual, a fused shortcut, GroupNorm statistics, up_time 2 and the "
+                  "OUT_F32, W_PER_BATCH, X_SHARED, BIAS_ALONG_M and FORCE_DIRECT flags");
+  return CVVAE_OK;
+}
+
 int conv_tc_launch(const cvvae_conv_desc* d, cudaStream_t stream) {
+  const int relu_rc = conv_relu_check(d);
+  if (relu_rc != CVVAE_OK) return relu_rc;
   ConvTcParams p;
   size_t smem = 0;
   long long grid = 0;
@@ -945,6 +980,14 @@ int conv_tc_launch(const cvvae_conv_desc* d, cudaStream_t stream) {
   }
 
   int rc = CVVAE_OK;
+  if (d->flags & CVVAE_CONV_RELU) {   // fp32 only (conv_relu_check)
+    if (N_cta == 256) rc = launch_bn<CVVAE_F32, 256, true>(tmA, tmB, tmA2, tmB2, tmY, tmR, p, static_cast<unsigned>(grid), smem, stream);
+    else if (N_cta == 128) rc = launch_bn<CVVAE_F32, 128, true>(tmA, tmB, tmA2, tmB2, tmY, tmR, p, static_cast<unsigned>(grid), smem, stream);
+    else rc = launch_bn<CVVAE_F32, 64, true>(tmA, tmB, tmA2, tmB2, tmY, tmR, p, static_cast<unsigned>(grid), smem, stream);
+    if (rc != CVVAE_OK) return rc;
+    CVVAE_LAUNCH_CHECK();
+    return CVVAE_OK;
+  }
   CVVAE_DISPATCH_DTYPE(d->dtype, {
     if (N_cta == 256) rc = launch_bn<DT, 256>(tmA, tmB, tmA2, tmB2, tmY, tmR, p, static_cast<unsigned>(grid), smem, stream);
     else if (N_cta == 128) rc = launch_bn<DT, 128>(tmA, tmB, tmA2, tmB2, tmY, tmR, p, static_cast<unsigned>(grid), smem, stream);

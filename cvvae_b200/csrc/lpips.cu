@@ -1,0 +1,243 @@
+// LPIPS (Zhang et al. 2018, VGG16 variant) of two uint8 videos, the learned perceptual distance the reference adds to its
+// reconstruction loss per frame (lvdm/modules/autoencoding/losses/discriminator_loss.py:239-256,
+// lvdm/modules/autoencoding/lpips/loss/lpips.py).  The thirteen 3 x 3 convolutions run on the tensor-core convolution
+// (conv_tc, fp32 activations, TF32 products, ReLU in its epilogue); this file holds the two kernels around them:
+//
+//   lpips_input_kernel: uint8 frames of both videos -> the scaled input of conv1_1 with its nine spatial taps packed
+//     into 32 channels, so that conv1_1 runs as a 1 x 1 convolution (as the engine runs conv_in).  A CTA first builds
+//     the 3 x 256 table of scaled byte values, which are all the values the input can take.
+//   lpips_tap_kernel: one tap (relu1_2 .. relu5_3) of both videos -> per frame, the sum over positions of
+//     sum_c w[c] (f_a / (|f_a| + eps) - f_b / (|f_b| + eps))^2, and optionally the 2 x 2 max pool of every image for the
+//     next block, in the same pass, rounded to the nearest TF32 value like every input of a convolution here.  One warp
+//     scores one position at a time (each lane holds C / 32 channels), walking 2 x 2 quads so that a full quad's pooled
+//     maximum is formed in registers on the way.
+//
+// The normalisation and the difference are fp64: a good reconstruction's f_a / |f_a| - f_b / |f_b| is small next to
+// either term, and fp32 would leave a relative error of 1e-7 / |difference| in it.  Accumulation: a warp keeps one
+// fp64 partial per lane over its positions, a CTA reduces its warps in a fixed order and adds its sum, rounded once to
+// units of 2^-32, to the frame's int64 with an integer atomic.  The CTA -> positions map depends on H and W alone, so a
+// frame's result is bit-reproducible and independent of the other frames in the call; identical frames give exactly 0
+// and swapping the videos gives the same bits (the expression is symmetric in a and b, term by term).
+#include <math.h>
+
+#include "common.cuh"
+
+namespace cvvae {
+
+constexpr int kLpInThreads = 256;
+constexpr int kLpInChannels = 32;     // 27 taps x channels, padded to a channel block of fp32 storage
+constexpr int kLpTapThreads = 256;
+constexpr int kLpQuadsPerWarp = 4;
+constexpr int kLpQuadsPerCta = kLpQuadsPerWarp * kLpTapThreads / 32;
+constexpr long long kLpMaxPositions = 1ll << 23;   // H * W of one tap: with |w| <= 32 the frame sum stays below 2^62 / 2^32
+
+// (x - shift) / scale of ScalingLayer (lpips.py:67-78), x = byte / 127.5 - 1, each operation one fp32 rounding as PyTorch
+// evaluates it, then rounded to the nearest TF32 value: the input's only consumer is a tensor-core product.
+__device__ __forceinline__ float lpips_scaled(int byte, int c) {
+  const float shift = c == 0 ? -0.030f : c == 1 ? -0.088f : -0.188f;
+  const float scale = c == 0 ? 0.458f : c == 1 ? 0.448f : 0.450f;
+  const float x = __fsub_rn(__fdiv_rn(static_cast<float>(byte), 127.5f), 1.0f);
+  return tf32_rn(__fdiv_rn(__fsub_rn(x, shift), scale));
+}
+
+// out [2T, H, W, 32]: image i < T is frame i of a, image T + i frame i of b; channel (kh*3 + kw)*3 + c of position
+// (h, w) is the scaled pixel (h + kh - 1, w + kw - 1, c), 0 outside the frame (conv2d pads the scaled input with zeros),
+// channels 27..31 are 0.  One thread per output position: 32 floats, eight 16-byte stores.
+__global__ void __launch_bounds__(kLpInThreads)
+    lpips_input_kernel(const uint8_t* __restrict__ a, const uint8_t* __restrict__ b, int T, int H, int W,
+                       float* __restrict__ out) {
+  __shared__ float s_tab[3][256];
+  for (int i = threadIdx.x; i < 3 * 256; i += kLpInThreads) s_tab[i >> 8][i & 255] = lpips_scaled(i & 255, i >> 8);
+  __syncthreads();
+  const long long n = 2ll * T * H * W;
+  const long long pos = static_cast<long long>(blockIdx.x) * kLpInThreads + threadIdx.x;
+  if (pos >= n) return;
+  const int w = static_cast<int>(pos % W);
+  const long long r = pos / W;
+  const int h = static_cast<int>(r % H);
+  const int img = static_cast<int>(r / H);
+  const uint8_t* src = (img < T ? a + static_cast<long long>(img) * H * W * 3 : b + static_cast<long long>(img - T) * H * W * 3);
+  float v[kLpInChannels];
+#pragma unroll
+  for (int kh = 0; kh < 3; ++kh)
+#pragma unroll
+    for (int kw = 0; kw < 3; ++kw) {
+      const int y = h + kh - 1, x = w + kw - 1;
+      const bool in = y >= 0 && y < H && x >= 0 && x < W;
+      const uint8_t* px = src + (static_cast<long long>(y) * W + x) * 3;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) v[(kh * 3 + kw) * 3 + c] = in ? s_tab[c][px[c]] : 0.f;
+    }
+#pragma unroll
+  for (int c = 27; c < kLpInChannels; ++c) v[c] = 0.f;
+  float4* dst = reinterpret_cast<float4*>(out + pos * kLpInChannels);
+#pragma unroll
+  for (int i = 0; i < kLpInChannels / 4; ++i) dst[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
+}
+
+// kV consecutive channels of one position, lane l holding [l*kV, l*kV + kV)
+template <int kV>
+__device__ __forceinline__ void lp_load(const float* p, float (&v)[kV]) {
+  if constexpr (kV == 2) {
+    const float2 q = __ldg(reinterpret_cast<const float2*>(p));
+    v[0] = q.x;
+    v[1] = q.y;
+  } else {
+#pragma unroll
+    for (int i = 0; i < kV / 4; ++i) {
+      const float4 q = __ldg(reinterpret_cast<const float4*>(p) + i);
+      v[4 * i] = q.x;
+      v[4 * i + 1] = q.y;
+      v[4 * i + 2] = q.z;
+      v[4 * i + 3] = q.w;
+    }
+  }
+}
+template <int kV>
+__device__ __forceinline__ void lp_store(float* p, const float (&v)[kV]) {
+  if constexpr (kV == 2) {
+    *reinterpret_cast<float2*>(p) = make_float2(v[0], v[1]);
+  } else {
+#pragma unroll
+    for (int i = 0; i < kV / 4; ++i)
+      reinterpret_cast<float4*>(p)[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
+  }
+}
+
+__device__ __forceinline__ double warp_sum(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// f [2T, H, W, C] (frames of a, then of b); acc[t] += sum over the frame's positions of the weighted squared difference
+// of the normalised features, in units of 2^-32.  pooled (optional) [2T, H/2, W/2, C]: 2 x 2 max pool, floor, rounded to
+// TF32 (rounding is monotonic, so this is the rounded max of the four values).
+// CTA (t, blk) owns quads [blk * 32, blk * 32 + 32) of frame t in row-major quad order; warp w of it quads 4w .. 4w + 3.
+// Two CTAs per SM at least below C = 512: left to itself ptxas gives C = 64 / 128 48 / 64 registers and spills.
+template <int C>
+__global__ void __launch_bounds__(kLpTapThreads, C >= 512 ? 1 : 2)
+    lpips_tap_kernel(const float* __restrict__ f, int T, int H, int W, const float* __restrict__ lin_w,
+                     unsigned long long* __restrict__ acc, float* __restrict__ pooled, int ctas_per_frame) {
+  constexpr int kV = C / 32;
+  __shared__ double s_red[kLpTapThreads / 32];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int t = blockIdx.x / ctas_per_frame, blk = blockIdx.x % ctas_per_frame;
+  const int QW = (W + 1) / 2, QH = (H + 1) / 2, PH = H / 2, PW = W / 2;
+  const long long img_stride = static_cast<long long>(H) * W * C;
+  const float* fa = f + static_cast<long long>(t) * img_stride + lane * kV;
+  const float* fb = f + static_cast<long long>(T + t) * img_stride + lane * kV;
+  double wc[kV];
+  {
+    float wf[kV];
+    lp_load<kV>(lin_w + lane * kV, wf);
+#pragma unroll
+    for (int i = 0; i < kV; ++i) wc[i] = wf[i];
+  }
+  double part = 0.0;
+  for (int i = 0; i < kLpQuadsPerWarp; ++i) {
+    const long long q = static_cast<long long>(blk) * kLpQuadsPerCta + warp * kLpQuadsPerWarp + i;
+    if (q >= static_cast<long long>(QH) * QW) break;   // warp-uniform
+    const int qh = static_cast<int>(q / QW), qw = static_cast<int>(q % QW);
+    const bool full = qh < PH && qw < PW;
+    float ma[kV], mb[kV];
+#pragma unroll
+    for (int k = 0; k < kV; ++k) ma[k] = mb[k] = -INFINITY;
+#pragma unroll
+    for (int p = 0; p < 4; ++p) {
+      const int h = 2 * qh + (p >> 1), w = 2 * qw + (p & 1);
+      if (h >= H || w >= W) continue;   // warp-uniform: the last row / column of an odd extent
+      const long long off = (static_cast<long long>(h) * W + w) * C;
+      float va[kV], vb[kV];
+      lp_load<kV>(fa + off, va);
+      lp_load<kV>(fb + off, vb);
+      double sa = 0.0, sb = 0.0;
+#pragma unroll
+      for (int k = 0; k < kV; ++k) {
+        sa = fma(static_cast<double>(va[k]), static_cast<double>(va[k]), sa);
+        sb = fma(static_cast<double>(vb[k]), static_cast<double>(vb[k]), sb);
+      }
+      sa = warp_sum(sa);
+      sb = warp_sum(sb);
+      // f / (sqrt(sum f^2 + 1e-10) + 1e-10), lpips.py:141-143, as a product with the reciprocal
+      const double ra = 1.0 / (sqrt(sa + 1e-10) + 1e-10), rb = 1.0 / (sqrt(sb + 1e-10) + 1e-10);
+#pragma unroll
+      for (int k = 0; k < kV; ++k) {
+        const double d = static_cast<double>(va[k]) * ra - static_cast<double>(vb[k]) * rb;
+        part = fma(wc[k], d * d, part);
+        ma[k] = fmaxf(ma[k], va[k]);
+        mb[k] = fmaxf(mb[k], vb[k]);
+      }
+    }
+    if (pooled && full) {
+      const long long po = (static_cast<long long>(qh) * PW + qw) * C + lane * kV;
+      const long long pstride = static_cast<long long>(PH) * PW * C;
+#pragma unroll
+      for (int k = 0; k < kV; ++k) {
+        ma[k] = tf32_rn(ma[k]);
+        mb[k] = tf32_rn(mb[k]);
+      }
+      lp_store<kV>(pooled + static_cast<long long>(t) * pstride + po, ma);
+      lp_store<kV>(pooled + static_cast<long long>(T + t) * pstride + po, mb);
+    }
+  }
+  part = warp_sum(part);
+  if (lane == 0) s_red[warp] = part;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+#pragma unroll
+    for (int i = 0; i < kLpTapThreads / 32; ++i) s += s_red[i];
+    atomicAdd(acc + t, static_cast<unsigned long long>(__double2ll_rn(s * 4294967296.0)));
+  }
+}
+
+}  // namespace cvvae
+
+using namespace cvvae;
+
+extern "C" int cvvae_lpips_input(const uint8_t* a_thwc, const uint8_t* b_thwc, int32_t T, int32_t H, int32_t W, float* out,
+                                 void* stream) {
+  CVVAE_CHECK_ARG(a_thwc && b_thwc && out, "cvvae_lpips_input: null pointer");
+  CVVAE_CHECK_ARG(T >= 0 && H >= 1 && W >= 1, "cvvae_lpips_input: needs T >= 0 and H, W >= 1, got T=%d H=%d W=%d", (int)T,
+                  (int)H, (int)W);
+  CVVAE_CHECK_ARG(reinterpret_cast<uintptr_t>(out) % 16 == 0, "cvvae_lpips_input: `out` must be 16-byte aligned");
+  if (T == 0) return CVVAE_OK;
+  const long long grid = (2ll * T * H * W + kLpInThreads - 1) / kLpInThreads;
+  CVVAE_CHECK_ARG(grid < (1ll << 31), "cvvae_lpips_input: too many positions for one launch (T=%d at %d x %d)", (int)T,
+                  (int)H, (int)W);
+  lpips_input_kernel<<<static_cast<unsigned>(grid), kLpInThreads, 0, static_cast<cudaStream_t>(stream)>>>(a_thwc, b_thwc, T,
+                                                                                                         H, W, out);
+  CVVAE_LAUNCH_CHECK();
+  return CVVAE_OK;
+}
+
+extern "C" int cvvae_lpips_tap(const float* f, int32_t T, int32_t H, int32_t W, int32_t C, const float* lin_w, int64_t* acc,
+                               float* pooled, void* stream_) {
+  CVVAE_CHECK_ARG(f && lin_w && acc, "cvvae_lpips_tap: null pointer");
+  CVVAE_CHECK_ARG(C == 64 || C == 128 || C == 256 || C == 512, "cvvae_lpips_tap: C must be 64, 128, 256 or 512, got %d", (int)C);
+  CVVAE_CHECK_ARG(T >= 0 && H >= 1 && W >= 1, "cvvae_lpips_tap: needs T >= 0 and H, W >= 1, got T=%d H=%d W=%d", (int)T, (int)H,
+                  (int)W);
+  CVVAE_CHECK_ARG(!pooled || (H >= 2 && W >= 2), "cvvae_lpips_tap: pooling needs H, W >= 2, got %d x %d", (int)H, (int)W);
+  CVVAE_CHECK_ARG(1ll * H * W <= kLpMaxPositions,
+                  "cvvae_lpips_tap: %d x %d positions exceed the 64-bit accumulator's range (H*W <= 2^23)", (int)H, (int)W);
+  CVVAE_CHECK_ARG(reinterpret_cast<uintptr_t>(f) % 16 == 0 && reinterpret_cast<uintptr_t>(lin_w) % 16 == 0 &&
+                      reinterpret_cast<uintptr_t>(pooled) % 16 == 0,
+                  "cvvae_lpips_tap: f, lin_w and pooled must be 16-byte aligned");
+  if (T == 0) return CVVAE_OK;
+  const long long quads = 1ll * ((H + 1) / 2) * ((W + 1) / 2);
+  const long long per_frame = (quads + kLpQuadsPerCta - 1) / kLpQuadsPerCta;
+  const long long grid = per_frame * T;
+  CVVAE_CHECK_ARG(grid < (1ll << 31), "cvvae_lpips_tap: too many frames for one launch (T=%d at %d x %d)", (int)T, (int)H, (int)W);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  CVVAE_CUDA(cudaMemsetAsync(acc, 0, sizeof(int64_t) * T, stream));
+  unsigned long long* out = reinterpret_cast<unsigned long long*>(acc);
+  const unsigned g = static_cast<unsigned>(grid);
+  const int pf = static_cast<int>(per_frame);
+  if (C == 64) lpips_tap_kernel<64><<<g, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, out, pooled, pf);
+  else if (C == 128) lpips_tap_kernel<128><<<g, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, out, pooled, pf);
+  else if (C == 256) lpips_tap_kernel<256><<<g, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, out, pooled, pf);
+  else lpips_tap_kernel<512><<<g, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, out, pooled, pf);
+  CVVAE_LAUNCH_CHECK();
+  return CVVAE_OK;
+}

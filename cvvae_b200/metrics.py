@@ -1,7 +1,8 @@
-"""Reconstruction quality on the GPU: per-frame PSNR, SSIM and multi-scale SSIM of two uint8 videos.
+"""Reconstruction quality on the GPU: per-frame PSNR, SSIM, multi-scale SSIM and LPIPS of two uint8 videos.
 
     frame_metrics(a, b)  ->  FrameMetrics(psnr, ssim, sse), host tensors with one entry per frame
     frame_ms_ssim(a, b)  ->  float64 host tensor with one MS-SSIM per frame
+    LPIPS.from_state_dict(*state_dicts)(a, b)  ->  float64 host tensor with one LPIPS per frame
 
 `a` and `b` are CUDA uint8 tensors [T, H, W, 3]: typically the frames the network saw (after the script's resize,
 cvvae_inference_video.py:28) and the frames it gave back (:47-50).  One kernel (`csrc/metrics.cu`) reads both once and
@@ -28,6 +29,20 @@ data_range=255, size_average=False)`` on [T, 3, H, W]; torchmetrics' MS-SSIM dif
 instead of padding, and it averages the channels before taking the product.  Level 4 must hold the window, so frames
 need at least 161 px on each side.  The pooled levels are kept as exact integer sums on the device, and one scoring
 kernel per level leaves the sums of cs and SSIM per channel in units of 2^-32; the product is taken on the host in float64.
+
+LPIPS (Zhang et al. 2018; the VGG16 variant, lpips v0.1) is the learned perceptual distance the reference adds to its
+reconstruction loss, per frame.  Per frame pair: s = ((frame / 127.5 - 1) - shift) / scale (fp32, shift = (-0.030,
+-0.088, -0.188), scale = (0.458, 0.448, 0.450)); VGG16 ``features[0:30]``, thirteen 3 x 3 convolutions (zero padding 1)
+each followed by ReLU, with a 2 x 2 max pool after convolutions 2, 4, 7 and 10; at the five taps relu1_2 .. relu5_3
+(C = 64, 128, 256, 512, 512), f^ = f / (sqrt(sum_c f^2 + 1e-10) + 1e-10) and d_k = mean over positions of
+sum_c w_k[c] (f^_a - f^_b)^2 with the 1 x 1 head lin{k}; LPIPS = sum_k d_k.  The convolutions run on the tensor-core
+convolution with fp32 activations and TF32 products, which is how PyTorch computes an fp32 LPIPS on this GPU by default
+(cuDNN with TF32 on); every activation that only a convolution reads is stored rounded to the nearest TF32 value, the
+taps stay fp32.  The normalisation and the weighted difference are fp64 and their per-frame sums integer fixed
+point, so results are bit-reproducible, independent of how frames are grouped, exactly 0 for identical frames and
+symmetric in a and b.  Frames need at least 16 x 16 px (relu5_3 is H/16 x W/16) and at most 2^23 px (the range of the
+fixed-point sums).  No weights ship with the package:
+``LPIPS.from_state_dict`` takes torchvision's VGG16 state dict (or the reference module's) and the lpips heads.
 """
 from __future__ import annotations
 
@@ -41,6 +56,16 @@ _WINDOW = 11
 MS_SSIM_WEIGHTS = (0.0448, 0.2856, 0.3001, 0.2363, 0.1333)
 MS_SSIM_MIN_SIZE = 161
 MS_SSIM_LAUNCHES = 9          # per call: five levels scored, four pooling steps
+LPIPS_MIN_SIZE = 16
+LPIPS_LAUNCHES = 19           # per group of frames: the input kernel, 13 convolutions, 5 taps
+LPIPS_MAX_POSITIONS = 1 << 23   # H * W: the range of the tap kernel's fixed-point sums (include/cvvae_b200.h)
+LPIPS_GROUP_BYTES = 8 << 30   # device bytes of VGG activations one group may take: one frame pair at the largest size
+LPIPS_SHIFT = (-0.030, -0.088, -0.188)
+LPIPS_SCALE = (0.458, 0.448, 0.450)
+LPIPS_MAX_HEAD = 32.0         # |w| bound of the heads that keeps the tap kernel's fixed-point sums in range
+# vgg16.features indices of the thirteen convolutions, per block (the reference's slice1 .. slice5); each block ends in a tap
+_VGG_BLOCKS = ((0, 2), (5, 7), (10, 12, 14), (17, 19, 21), (24, 26, 28))
+_VGG_CHANNELS = (64, 128, 256, 512, 512)
 
 
 class FrameMetrics(NamedTuple):
@@ -136,3 +161,173 @@ def frame_ms_ssim(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
     if T == 0:
         return torch.empty(0, dtype=torch.float64)
     return _ms_ssim_scores(_launch_ms_ssim(a.contiguous(), b.contiguous()).cpu(), H, W)
+
+
+def _check_lpips_size(H: int, W: int, who: str) -> None:
+    if min(H, W) < LPIPS_MIN_SIZE:
+        raise ValueError(f"{who}: LPIPS needs frames of at least {LPIPS_MIN_SIZE} x {LPIPS_MIN_SIZE} px (its last tap, "
+                         f"relu5_3, is 1/16 of the size); got {H} x {W}")
+    if H * W > LPIPS_MAX_POSITIONS:
+        raise ValueError(f"{who}: LPIPS takes frames of at most 2^23 px (the range of its fixed-point sums); got {H} x {W}")
+
+
+def _lpips_tap_sizes(H: int, W: int) -> list:
+    """(h, w) of the five taps: each block after the first starts with a 2 x 2 max pool, floor."""
+    return [(H >> k, W >> k) for k in range(len(_VGG_BLOCKS))]
+
+
+def _lpips_scores(acc: torch.Tensor, H: int, W: int) -> torch.Tensor:
+    """Host int64 [5, T] of the tap kernels (per tap and frame, the sum over positions times 2^32) -> LPIPS, float64 [T]."""
+    d = torch.zeros(acc.shape[1], dtype=torch.float64)
+    for k, (h, w) in enumerate(_lpips_tap_sizes(H, W)):
+        d += acc[k].double() / 4294967296.0 / (h * w)
+    return d
+
+
+def _lpips_weights(state_dicts: tuple) -> tuple:
+    """The checked weights of ``LPIPS.from_state_dict`` on the host, fp32: ([(weight, bias)] of the thirteen
+    convolutions, [head [C_k]] of the five taps)."""
+    sd: dict = {}
+    for d in state_dicts:
+        sd.update(d)
+
+    def get(keys: tuple, shape: tuple) -> torch.Tensor:
+        key = next((k for k in keys if k in sd), None)
+        if key is None:
+            raise ValueError(f"LPIPS.from_state_dict: missing key {keys[0]!r}" +
+                             (f" (or {keys[1]!r})" if len(keys) > 1 else ""))
+        v = sd[key]
+        v = torch.as_tensor(v) if not isinstance(v, torch.Tensor) else v.detach()
+        if tuple(v.shape) != shape:
+            raise ValueError(f"LPIPS.from_state_dict: {key!r} has shape {tuple(v.shape)}, expected {shape}")
+        if not v.is_floating_point():
+            raise ValueError(f"LPIPS.from_state_dict: {key!r} is {v.dtype}, expected a floating-point tensor")
+        v = v.to("cpu", torch.float32)
+        if not torch.isfinite(v).all():
+            raise ValueError(f"LPIPS.from_state_dict: {key!r} has non-finite values")
+        return v
+
+    for name, want in (("shift", LPIPS_SHIFT), ("scale", LPIPS_SCALE)):
+        key = f"scaling_layer.{name}"
+        if key in sd:
+            v = get((key,), (1, 3, 1, 1))
+            if not torch.equal(v.flatten(), torch.tensor(want, dtype=torch.float32)):
+                raise ValueError(f"LPIPS.from_state_dict: {key!r} is {v.flatten().tolist()}, expected {list(want)}")
+    convs = []
+    cin = 3
+    for k, (block, c) in enumerate(zip(_VGG_BLOCKS, _VGG_CHANNELS)):
+        for i in block:
+            keys = lambda s: (f"features.{i}.{s}", f"net.slice{k + 1}.{i}.{s}")   # noqa: E731
+            convs.append((get(keys("weight"), (c, cin, 3, 3)), get(keys("bias"), (c,))))
+            cin = c
+    heads = []
+    for k, c in enumerate(_VGG_CHANNELS):
+        key = f"lin{k}.model.1.weight"
+        v = get((key,), (1, c, 1, 1))
+        if v.abs().max().item() > LPIPS_MAX_HEAD:
+            raise ValueError(f"LPIPS.from_state_dict: {key!r} has |w| > {LPIPS_MAX_HEAD:g}, outside the range of the "
+                             "fixed-point sums")
+        heads.append(v.flatten())
+
+    return convs, heads
+
+
+class LPIPS:
+    """LPIPS (VGG16, lpips v0.1) of every frame of `b` against the same frame of `a` on the GPU; the module docstring has
+    the definition.  Build it with ``LPIPS.from_state_dict``; ``metric(a, b)`` takes two CUDA uint8 ``[T, H, W, 3]``
+    videos on ``metric.device`` (H, W >= 16, H * W <= 2^23) and returns float64 ``[T]`` on the host.
+
+    Frames are scored in groups whose VGG activations stay within ``LPIPS_GROUP_BYTES``; each group is
+    ``LPIPS_LAUNCHES`` kernel launches on the current stream of the device.  The result is the same, bit for bit,
+    whatever the grouping."""
+
+    def __init__(self, blocks: list, heads: list, device: torch.device):
+        from .ops import CudaOps
+        self._ops = CudaOps()
+        self._blocks = blocks          # per block: [(packed weight, bias, 1 x 1 tap-packed?)]
+        self._heads = heads            # fp32 [C_k] per tap
+        self.device = device
+        self._group_bytes = LPIPS_GROUP_BYTES
+
+    @classmethod
+    def from_state_dict(cls, *state_dicts, device=None) -> "LPIPS":
+        """Weights from one or more state dicts, merged (later ones win): the thirteen convolutions under torchvision's
+        keys ``features.{i}.weight`` / ``.bias`` (``vgg16-397923af.pth``) or the reference module's ``net.slice{k}.{i}.*``
+        (same i), the heads under ``lin{k}.model.1.weight`` ``[1, C_k, 1, 1]`` (lpips v0.1 ``vgg.pth``, or the reference's
+        ``LPIPS().state_dict()``).  ``scaling_layer.shift`` / ``.scale``, if present, must be the constants above; every
+        other key is ignored.  A missing key, a wrong shape, a non-float or non-finite value, or a head with |w| > 32
+        raises ValueError.  `device`: a CUDA device (default: the current one).  The weights are packed once, the
+        convolutions' rounded to TF32."""
+        convs, heads = _lpips_weights(state_dicts)
+        dev = torch.device(device) if device is not None else None
+        if dev is not None and dev.type != "cuda":
+            raise ValueError(f"LPIPS.from_state_dict: the device must be a CUDA device, got {dev}")
+        if dev is None or dev.index is None:
+            dev = torch.device("cuda", torch.cuda.current_device() if dev is None or dev.index is None else dev.index)
+        from .ops import CudaOps
+        ops = CudaOps()
+        blocks, n = [], 0
+        for k, block in enumerate(_VGG_BLOCKS):
+            layers = []
+            for _ in block:
+                w, b = convs[n]
+                if n == 0:   # conv1_1 as a 1 x 1 convolution over the 32 tap-packed channels of cvvae_lpips_input
+                    wp = torch.zeros((w.shape[0], 32), dtype=torch.float32)
+                    wp[:, :27] = w.permute(0, 2, 3, 1).reshape(w.shape[0], 27)
+                    w = wp[:, :, None, None]
+                layers.append((ops.pack_weight(w.to(dev).contiguous()), b.to(dev), n == 0))
+                n += 1
+            blocks.append(layers)
+        m = cls(blocks, [h.to(dev) for h in heads], dev)
+        return m
+
+    def _group(self, H: int, W: int) -> int:
+        """Frames per group: the largest activations live at once are conv1_2's input and output, 64 + 64 fp32 channels
+        at full size for both videos."""
+        return max(1, self._group_bytes // (2 * 128 * 4 * H * W))
+
+    @L._on_tensor_device
+    def _launch(self, a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
+        """The kernels on the current stream of the frames' device: int64 [5, T] (per tap and frame, the sum over
+        positions of the weighted squared difference times 2^32), on the device."""
+        T, H, W, _ = a.shape
+        acc = torch.empty((len(_VGG_BLOCKS), T), dtype=torch.int64, device=a.device)
+        g = self._group(H, W)
+        for t0 in range(0, T, g):
+            self._run_group(a[t0:t0 + g], b[t0:t0 + g], acc[:, t0:t0 + g])
+        return acc
+
+    def _run_group(self, a: torch.Tensor, b: torch.Tensor, acc: torch.Tensor) -> None:
+        G, H, W, _ = a.shape
+        lib, dev, stream = self._ops.lib, a.device, L._stream(a)
+        x = torch.empty((2 * G, 1, H, W, 32), dtype=torch.float32, device=dev)
+        L.check(lib.cvvae_lpips_input(a.data_ptr(), b.data_ptr(), G, H, W, x.data_ptr(), stream), "cvvae_lpips_input")
+        h, w = H, W
+        for k, layers in enumerate(self._blocks):
+            for j, (wp, bias, packed_taps) in enumerate(layers):
+                y = torch.empty((2 * G, 1, h, w, wp.shape[1]), dtype=torch.float32, device=dev)
+                # a block's last convolution is a tap, read as data in fp32; the others only feed the next convolution
+                # and are stored rounded to TF32, as the tensor cores should read them
+                kw = dict(relu=True, tf32_out=j + 1 < len(layers))
+                if packed_taps:
+                    self._ops.conv(x, wp, bias, out=y, **kw)
+                else:
+                    self._ops.conv(x, wp, bias, kernel=(1, 3, 3), offset=(0, -1, -1), out=y, **kw)
+                x = y
+            C = x.shape[-1]
+            pooled = (torch.empty((2 * G, 1, h // 2, w // 2, C), dtype=torch.float32, device=dev)
+                      if k + 1 < len(self._blocks) else None)
+            L.check(lib.cvvae_lpips_tap(x.data_ptr(), G, h, w, C, self._heads[k].data_ptr(), acc[k].data_ptr(),
+                                        None if pooled is None else pooled.data_ptr(), stream), "cvvae_lpips_tap")
+            if pooled is not None:
+                x, h, w = pooled, h // 2, w // 2
+
+    def __call__(self, a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
+        _check_frames(a, b, "LPIPS")
+        if a.device != self.device:
+            raise ValueError(f"LPIPS: the frames are on {a.device}, the weights on {self.device}")
+        T, H, W, _ = a.shape
+        _check_lpips_size(H, W, "LPIPS")
+        if T == 0:
+            return torch.empty(0, dtype=torch.float64)
+        return _lpips_scores(self._launch(a.contiguous(), b.contiguous()).cpu(), H, W)

@@ -95,17 +95,21 @@ class CudaOps:
              out_f32: bool = False, bias_along_m: bool = False, w_ld: int = 0, cout: Optional[int] = None,
              force: Optional[str] = None, ref_taps: Optional[int] = None, gn_stats: Optional[torch.Tensor] = None,
              gn_groups: int = 32, w_per_batch: bool = False, x_shared: bool = False,
-             k_alg: Optional[int] = None, sc_x: Optional[torch.Tensor] = None, sc_w: Optional[torch.Tensor] = None) -> torch.Tensor:
+             k_alg: Optional[int] = None, sc_x: Optional[torch.Tensor] = None, sc_w: Optional[torch.Tensor] = None,
+             relu: bool = False, tf32_out: bool = False) -> torch.Tensor:
         """y = alpha * conv(x, w) + bias + residual.  ``w`` is packed [taps, Cout, Cin(ld)].
 
         Batched GEMM (attention): ``w_per_batch`` - w is [B, Cout, Cin(ld)], one matrix per batch item of y;
         ``x_shared`` - x has batch 1 and is the left operand of every batch item.
         Fused 1x1 shortcut: ``sc_x`` [B,T,H,W,C2] (the output's extents) times ``sc_w`` [Cout, C2] is accumulated into the
-        same fp32 accumulators as the taps (``bias`` then carries the sum of both biases)."""
+        same fp32 accumulators as the taps (``bias`` then carries the sum of both biases).
+        ``relu``: y = max(alpha * conv(x, w) + bias, 0) in the epilogue (fp32, tensor-core path, no residual; CVVAE_CONV_RELU),
+        with ``tf32_out`` stored rounded to the nearest TF32 value (an output only tensor-core products read)."""
         d = self._conv_desc(x, w, bias, kernel=kernel, stride=stride, offset=offset, pad_t=pad_t, pad_hw=pad_hw,
                             up_time=up_time, residual=residual, alpha=alpha, out=out, out_f32=out_f32,
                             bias_along_m=bias_along_m, w_ld=w_ld, cout=cout, gn_stats=gn_stats, gn_groups=gn_groups,
-                            w_per_batch=w_per_batch, x_shared=x_shared, sc_x=sc_x, sc_w=sc_w)
+                            w_per_batch=w_per_batch, x_shared=x_shared, sc_x=sc_x, sc_w=sc_w, relu=relu,
+                            tf32_out=tf32_out)
         B, T, H, W, Ci = x.shape
         if x_shared:
             B = out.shape[0]
@@ -165,7 +169,8 @@ class CudaOps:
     @staticmethod
     def _conv_desc(x, w, bias, *, kernel=(1, 1, 1), stride=(1, 1, 1), offset=(0, 0, 0), pad_t=L.PAD_ZERO, pad_hw=L.PAD_ZERO,
                    up_time=1, residual=None, alpha=1.0, out=None, out_f32=False, bias_along_m=False, w_ld=0, cout=None,
-                   gn_stats=None, gn_groups=32, w_per_batch=False, x_shared=False, sc_x=None, sc_w=None) -> L.ConvDesc:
+                   gn_stats=None, gn_groups=32, w_per_batch=False, x_shared=False, sc_x=None, sc_w=None,
+                   relu=False, tf32_out=False) -> L.ConvDesc:
         kt, kh, kw = kernel
         st, sh, sw = stride
         ot, oh, ow = offset
@@ -190,7 +195,8 @@ class CudaOps:
         d.up_time = up_time
         d.dtype = dtype_code(x.dtype)
         d.flags = ((L.CONV_BIAS_ALONG_M if bias_along_m else 0) | (L.CONV_OUT_F32 if out_f32 else 0) |
-                   (L.CONV_W_PER_BATCH if w_per_batch else 0) | (L.CONV_X_SHARED if x_shared else 0))
+                   (L.CONV_W_PER_BATCH if w_per_batch else 0) | (L.CONV_X_SHARED if x_shared else 0) |
+                   (L.CONV_RELU if relu else 0) | (L.CONV_TF32_OUT if tf32_out else 0))
         d.alpha = alpha
         if gn_stats is not None:  # int64 fixed point [B, groups, 2], zeroed by the caller; the epilogue accumulates into it
             assert gn_stats.dtype == torch.int64 and gn_stats.is_contiguous()

@@ -11,7 +11,8 @@ chunk however long the clip is, and the concatenated chunks are bit-identical to
 
 ``reconstruct_frames`` chains pixel upload, encoder, posterior, decoder and pixel download over host uint8 frames:
 the body of the reference's ``cvvae_inference_video.py`` as a stream.  ``evaluate_frames`` is the same stream with every
-reconstructed frame scored (PSNR, SSIM, optionally MS-SSIM) on the device against the input frame the network saw.
+reconstructed frame scored (PSNR, SSIM, optionally MS-SSIM and LPIPS) on the device against the input frame the network
+saw.
 
 ``encode_clips`` turns a dataset of clips into latents: each clip goes through the reference's training pre-processing
 (``video_io.frames_to_training_input``) straight into its slot of a batch, and batches of clips with equal length run
@@ -230,13 +231,14 @@ def reconstruct_frames(model, frames: Iterable, size=None, sample_posterior: boo
     and bfloat16 models are supported (the pixel conversion kernels are 16-bit).
     """
     enc, dec = _open(model, "reconstruct_frames")
-    return _reconstruct(model, enc, dec, iter(frames), size, sample_posterior, generator, False, False)
+    return _reconstruct(model, enc, dec, iter(frames), size, sample_posterior, generator, False, False, None)
 
 
 def evaluate_frames(model, frames: Iterable, size=None, sample_posterior: bool = False,
-                    generator: Optional[torch.Generator] = None, *, ms_ssim: bool = False) -> Iterator[tuple]:
-    """``reconstruct_frames`` with a score for every frame: yields ``(frames_u8, psnr, ssim)`` per piece, and
-    ``(frames_u8, psnr, ssim, ms_ssim)`` with ``ms_ssim=True``.
+                    generator: Optional[torch.Generator] = None, *, ms_ssim: bool = False, lpips=None) -> Iterator[tuple]:
+    """``reconstruct_frames`` with a score for every frame: yields ``(frames_u8, psnr, ssim)`` per piece,
+    ``(frames_u8, psnr, ssim, ms_ssim)`` with ``ms_ssim=True``, and the per-frame LPIPS as one more last element when
+    `lpips` is given.
 
     Same inputs and refusals as ``reconstruct_frames``, and ``frames_u8`` is what it yields.  ``psnr`` and ``ssim`` are
     float64 host tensors with one entry per frame of the piece (``cvvae_b200.metrics`` has the definitions).  Output
@@ -253,9 +255,22 @@ def evaluate_frames(model, frames: Iterable, size=None, sample_posterior: bool =
     ``metrics.MS_SSIM_LAUNCHES`` more kernels per piece on the same stream, right after the PSNR / SSIM kernel, on the
     same aligned input frames, and their sums ride in the same download.  MS-SSIM needs frames of at least 161 x 161 px
     as the network sees them; smaller ones raise ``ValueError`` when the first of them arrives.
+
+    `lpips`: a ``metrics.LPIPS`` on the model's device (another device raises ``ValueError`` at the call).  Each piece
+    is then also scored by LPIPS (float64 per frame): ``metrics.LPIPS_LAUNCHES`` kernels per group of frames on the same
+    stream, right after the other metric kernels, on the same aligned input frames; its sums ride in the same download.
+    The VGG activations of one group are freed before the next, so device memory stays flat in the clip's length.
+    LPIPS needs frames of at least 16 x 16 px as the network sees them; smaller ones raise ``ValueError`` when the first
+    of them arrives.
     """
+    from . import metrics
+    if lpips is not None:
+        if not isinstance(lpips, metrics.LPIPS):
+            raise ValueError(f"evaluate_frames: `lpips` must be a metrics.LPIPS or None; got {type(lpips).__name__}")
+        if lpips.device != model.device:
+            raise ValueError(f"evaluate_frames: the LPIPS weights are on {lpips.device}, the model on {model.device}")
     enc, dec = _open(model, "evaluate_frames")
-    return _reconstruct(model, enc, dec, iter(frames), size, sample_posterior, generator, True, bool(ms_ssim))
+    return _reconstruct(model, enc, dec, iter(frames), size, sample_posterior, generator, True, bool(ms_ssim), lpips)
 
 
 def _open(model, who: str):
@@ -267,9 +282,9 @@ def _open(model, who: str):
 
 
 def _reconstruct(model, enc: StreamEncoder, dec: StreamDecoder, frames: Iterator, size, sample_posterior: bool,
-                 generator, score: bool, ms_ssim: bool) -> Iterator:
+                 generator, score: bool, ms_ssim: bool, lpips) -> Iterator:
     """The stream behind reconstruct_frames (`score` False: yields frames) and evaluate_frames (True: yields
-    (frames, psnr, ssim), and (frames, psnr, ssim, ms_ssim) with `ms_ssim`)."""
+    (frames, psnr, ssim), then ms_ssim with `ms_ssim`, then the LPIPS with an `lpips` metric)."""
     from . import metrics
     from .video_io import frames_to_input, frames_to_input_and_u8, output_to_frames
 
@@ -303,18 +318,24 @@ def _reconstruct(model, enc: StreamEncoder, dec: StreamDecoder, frames: Iterator
             raise ValueError(f"evaluate_frames: the networks return {u8.shape[1]} x {u8.shape[2]} frames for an input of "
                              f"{ref.shape[1]} x {ref.shape[2]}, and frames of different sizes cannot be scored; pass "
                              "`size=` with a size the networks reproduce (a multiple of their spatial stride)")
+        sums = [metrics._launch(ref, u8)]
         if ms_ssim:
-            io.download(u8, metrics._launch(ref, u8), metrics._launch_ms_ssim(ref, u8))
-        else:
-            io.download(u8, metrics._launch(ref, u8))
+            sums.append(metrics._launch_ms_ssim(ref, u8))
+        if lpips is not None:
+            sums.append(lpips._launch(ref, u8))
+        io.download(u8, *sums)
 
-    def piece(host: torch.Tensor, sums: Optional[torch.Tensor] = None, ms_sums: Optional[torch.Tensor] = None):
+    def piece(host: torch.Tensor, sums: Optional[torch.Tensor] = None, *extra: torch.Tensor):
         if sums is None:
             return host
-        m = metrics._scores(sums, host.shape[1], host.shape[2])
-        if ms_sums is None:
-            return host, m.psnr, m.ssim
-        return host, m.psnr, m.ssim, metrics._ms_ssim_scores(ms_sums, host.shape[1], host.shape[2])
+        H, W = host.shape[1], host.shape[2]
+        m = metrics._scores(sums, H, W)
+        out = [host, m.psnr, m.ssim]
+        if ms_ssim:
+            out.append(metrics._ms_ssim_scores(extra[0], H, W))
+        if lpips is not None:
+            out.append(metrics._lpips_scores(extra[-1], H, W))
+        return tuple(out)
 
     def decode_chunks(latent_chunks) -> None:
         for post in latent_chunks:
@@ -327,9 +348,12 @@ def _reconstruct(model, enc: StreamEncoder, dec: StreamDecoder, frames: Iterator
         t = item.shape[0]
         if t == 0:
             continue
-        if ms_ssim:
-            metrics._check_ms_ssim_size(*((int(size[0]), int(size[1])) if size is not None else item.shape[1:3]),
-                                        "evaluate_frames")
+        if ms_ssim or lpips is not None:
+            seen = (int(size[0]), int(size[1])) if size is not None else tuple(item.shape[1:3])
+            if ms_ssim:
+                metrics._check_ms_ssim_size(*seen, "evaluate_frames")
+            if lpips is not None:
+                metrics._check_lpips_size(*seen, "evaluate_frames")
         dev_u8 = io.upload(item)
         if score:
             x, ref = frames_to_input_and_u8(dev_u8, dtype=model.dtype, size=size)

@@ -50,7 +50,18 @@ enum {
   /* Batched GEMM over the B axis (the per-frame attention products, models/vae_models.py:446-461,500-528): */
   CVVAE_CONV_W_PER_BATCH = 8,  /* `w` holds one [Cout][Cin(ld)] matrix PER batch item ([y.B][Cout][w_ld], contiguous);
                                   1x1x1 flat problems only.  A CVVAE_CONV_BIAS_ALONG_M bias is then [T*H*W], shared  */
-  CVVAE_CONV_X_SHARED = 16     /* x.B == 1: the same left operand for every batch item of y                       */
+  CVVAE_CONV_X_SHARED = 16,    /* x.B == 1: the same left operand for every batch item of y                       */
+  /* y = max(alpha * acc + bias, 0) (-0 stored as +0), in the register epilogue: the conv + ReLU pairs of VGG16's
+   * features[0:30] that LPIPS runs (lvdm/modules/autoencoding/lpips/loss/lpips.py:99-138).  CVVAE_F32 on the tensor-core
+   * path only; refused with CVVAE_E_ARG before any launch for 16-bit dtypes, by cvvae_conv3d_direct,
+   * cvvae_conv3d_stacked and by cvvae_conv3d on a descriptor the tensor-core path does not take, and together with a
+   * residual, x2 / w2, gn_stats, up_time 2 or any other flag but CVVAE_CONV_TF32_OUT.  cvvae_conv_tc_plan reports the
+   * same plan with it. */
+  CVVAE_CONV_RELU = 32,
+  /* With CVVAE_CONV_RELU only (refused otherwise, in the same places): y is stored rounded to the nearest TF32 value, for
+   * an output whose only consumers are tensor-core products (the VGG16 layers that are not LPIPS taps), which would
+   * otherwise read it with the low 13 mantissa bits dropped.  Same plan. */
+  CVVAE_CONV_TF32_OUT = 64
 };
 
 /* One strided channels-last 5-D tensor view. */
@@ -245,6 +256,36 @@ int cvvae_frame_ms_ssim(const uint8_t* a_thwc, const uint8_t* b_thwc, int32_t T,
                         int64_t* acc, void* stream);
 /* Bytes of the workspace cvvae_frame_ms_ssim needs for T frames of H x W px (T >= 0, H, W >= 1; else CVVAE_E_ARG). */
 int64_t cvvae_ms_ssim_workspace_bytes(int32_t T, int32_t H, int32_t W);
+
+/* LPIPS (VGG16, lpips v0.1) of two uint8 videos a, b: [T,H,W,3], contiguous, on the device, per frame:
+ * LPIPS.forward(input, target) of the reference in eval mode (lvdm/modules/autoencoding/lpips/loss/lpips.py:46-64), with the
+ * inputs taken as frame / 127.5 - 1.  The caller runs:
+ *   cvvae_lpips_input: out fp32 [2T,H,W,32] channels-last, 16-byte aligned; image i < T is frame i of a, image T+i frame i of
+ *     b.  Channel (kh*3 + kw)*3 + c of position (h, w) is s(h+kh-1, w+kw-1, c), s = ((p / 127.5 - 1) - shift_c) / scale_c
+ *     (ScalingLayer, lpips.py:67-78: shift = (-0.030, -0.088, -0.188), scale = (0.458, 0.448, 0.450)), every operation an
+ *     fp32 rounding as PyTorch evaluates it, stored rounded to the nearest TF32; 0 outside the frame (conv2d zero-pads the
+ *     scaled input) and in channels 27..31.  conv1_1 then runs as a 1 x 1 convolution over these 32 channels with its
+ *     weights packed [1][64][32] in the same channel order.  T >= 0 (T == 0 launches nothing), H, W >= 1.  One launch.
+ *   the thirteen 3 x 3 convolutions of vgg16.features[0:30] (lpips.py:99-138) through cvvae_conv3d with CVVAE_CONV_RELU, plus
+ *     CVVAE_CONV_TF32_OUT on the eight whose output only feeds the next convolution (all but the taps).
+ *   cvvae_lpips_tap on each of the five taps relu1_2 .. relu5_3: f fp32 [2T,H,W,C] (C = 64, 128, 256 or 512),
+ *     lin_w fp32 [C] (the 1x1 head lin{k}, no bias), acc int64 [T] overwritten with, per frame t,
+ *       acc[t] = 2^32 * sum over the positions of sum_c w[c] (fa_c / n_a - fb_c / n_b)^2,
+ *       n = sqrt(sum_c f_c^2 + 1e-10) + 1e-10   (normalize_tensor, lpips.py:141-143),
+ *     with fa = image t, fb = image T+t.  The normalisation and the difference are fp64; each CTA's fp64 sum over its
+ *     positions is rounded once to units of 2^-32 and added with an integer atomic: bit-reproducible, independent of the
+ *     other frames in the call, exactly 0 for identical frames and the same bits with a and b swapped.  Range: H*W <= 2^23
+ *     is checked (CVVAE_E_ARG); the heads must satisfy |w[c]| <= 32 (the Python loader refuses others; the entry point
+ *     cannot read device memory before it launches) and the features must be finite.  Then |acc[t]| < 2^62.
+ *     pooled: NULL, or fp32 [2T,H/2,W/2,C] that receives the 2 x 2 max pool (stride 2, floor) of all 2T images, the input
+ *     of the next block, from the same pass, stored rounded to the nearest TF32 value (its only consumer is a
+ *     convolution).  f, lin_w and pooled 16-byte aligned; T >= 0 (T == 0 launches nothing).
+ *     One launch (plus a memset of acc).
+ *   d_k(t) = acc[t] / 2^32 / (H_k W_k) and LPIPS(t) = sum_k d_k(t) are formed by the caller in fp64.  One group of frames
+ *   costs 1 + 13 + 5 kernel launches. */
+int cvvae_lpips_input(const uint8_t* a_thwc, const uint8_t* b_thwc, int32_t T, int32_t H, int32_t W, float* out, void* stream);
+int cvvae_lpips_tap(const float* f, int32_t T, int32_t H, int32_t W, int32_t C, const float* lin_w, int64_t* acc,
+                    float* pooled, void* stream);
 
 /* Diagnostics */
 /* Per-CTA phase timestamps of the next conv_tc launches: device buffer of n_ctas x 8 uint64 (globaltimer ns:

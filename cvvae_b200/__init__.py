@@ -8,8 +8,8 @@ Datasets of clips to latents, with the reference's training pre-processing (stre
     encode_clips, frames_to_training_input
 Datasets of clip latents back to uint8 videos, batched, in float16, bfloat16 or float32 (streaming.py, video_io.py):
     decode_clips, batch_to_frames
-Reconstruction quality on the device (cvvae_b200/metrics.py): per-frame PSNR / SSIM, multi-scale SSIM and LPIPS (VGG16,
-weights from a state dict) of uint8 videos, and the reconstruction stream with every frame scored (MS-SSIM with
+Reconstruction quality on the device (cvvae_b200/metrics.py): per-frame PSNR / SSIM, multi-scale SSIM and LPIPS (VGG16 or,
+with ``net="alex"``, AlexNet; weights from a state dict) of uint8 videos, and the reconstruction stream with every frame scored (MS-SSIM with
 ``ms_ssim=True``, LPIPS with ``lpips=LPIPS.from_state_dict(...)``):
     frame_metrics, FrameMetrics, frame_ms_ssim, LPIPS, evaluate_frames
 """

@@ -10,7 +10,12 @@
 //     sum_c w[c] (f_a / (|f_a| + eps) - f_b / (|f_b| + eps))^2, and optionally the 2 x 2 max pool of every image for the
 //     next block, in the same pass, rounded to the nearest TF32 value like every input of a convolution here.  One warp
 //     scores one position at a time (each lane holds C / 32 channels), walking 2 x 2 quads so that a full quad's pooled
-//     maximum is formed in registers on the way.
+//     maximum is formed in registers on the way.  lpips_tap_copy_kernel is the same pass writing, instead of the pool, a
+//     TF32-rounded copy of the tap for a convolution that reads it (AlexNet's relu3 and relu4).
+//
+// LPIPS on AlexNet features (net='alex') runs its five convolutions on conv_tc too; conv1 (11 x 11, stride 4) and conv2
+// (5 x 5) as 1 x 1 convolutions over their taps packed into channels by lpips_alex_input_kernel (from the uint8 frames,
+// 384 channels) and lpips_pack5x5_kernel (1600 channels), with lpips_max_pool3s2_kernel for the 3 x 3 stride-2 pools.
 //
 // The normalisation and the difference are fp64: a good reconstruction's f_a / |f_a| - f_b / |f_b| is small next to
 // either term, and fp32 would leave a relative error of 1e-7 / |difference| in it.  Accumulation: a warp keeps one
@@ -75,6 +80,88 @@ __global__ void __launch_bounds__(kLpInThreads)
   for (int i = 0; i < kLpInChannels / 4; ++i) dst[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
 }
 
+// AlexNet's conv1 (11 x 11, stride 4, zero padding 2, lpips net='alex') as a 1 x 1 convolution over its 3 * 11 * 11 = 363
+// taps, padded to 384 channels.  out [2T, OH, OW, 384], OH = (H - 7) / 4 + 1 (likewise OW): channel (c * 11 + kh) * 11 + kw
+// of position (oh, ow) is the scaled pixel (4 oh + kh - 2, 4 ow + kw - 2, c) as lpips_input_kernel computes it, 0 outside
+// the frame and in channels 363..383; the channel order is that of the PyTorch weight [64, 3, 11, 11] flattened.  One
+// thread per four channels of a position (one 16-byte store), so consecutive threads write consecutive bytes.  The index
+// within an image is 32-bit (the entry point checks OH * OW * 96 < 2^31), images are walked along y with 64-bit offsets.
+constexpr int kLpAlexK = 11;
+constexpr int kLpAlexTaps = 3 * kLpAlexK * kLpAlexK;
+constexpr int kLpAlexInChannels = 384;
+__global__ void __launch_bounds__(kLpInThreads)
+    lpips_alex_input_kernel(const uint8_t* __restrict__ a, const uint8_t* __restrict__ b, int T, int H, int W, int OH, int OW,
+                            float* __restrict__ out) {
+  __shared__ float s_tab[3][256];
+  for (int i = threadIdx.x; i < 3 * 256; i += kLpInThreads) s_tab[i >> 8][i & 255] = lpips_scaled(i & 255, i >> 8);
+  __syncthreads();
+  constexpr int kQ = kLpAlexInChannels / 4;
+  const int n = OH * OW * kQ;
+  const int i = blockIdx.x * kLpInThreads + threadIdx.x;
+  if (i >= n) return;
+  const int q = i % kQ, pos = i / kQ;
+  const int oh = pos / OW, ow = pos % OW;
+  for (int img = blockIdx.y; img < 2 * T; img += gridDim.y) {
+    const uint8_t* src = img < T ? a + static_cast<long long>(img) * H * W * 3 : b + static_cast<long long>(img - T) * H * W * 3;
+    float v[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int ch = 4 * q + j;
+      const int c = ch / (kLpAlexK * kLpAlexK), k = ch % (kLpAlexK * kLpAlexK);
+      const int y = 4 * oh + k / kLpAlexK - 2, x = 4 * ow + k % kLpAlexK - 2;
+      const bool in = ch < kLpAlexTaps && y >= 0 && y < H && x >= 0 && x < W;
+      v[j] = in ? s_tab[c][src[(static_cast<long long>(y) * W + x) * 3 + c]] : 0.f;
+    }
+    reinterpret_cast<float4*>(out + static_cast<long long>(img) * n * 4)[i] = make_float4(v[0], v[1], v[2], v[3]);
+  }
+}
+
+// 3 x 3 max pool, stride 2, no padding, floor (AlexNet's features[2] and [5]): out [N, OH, OW, C], OH = (H - 3) / 2 + 1, of
+// f [N, H, W, C], rounded to the nearest TF32 value (its only consumer is a convolution; rounding is monotonic, so this is
+// the pool of the rounded values).  One thread per four channels of an output position.
+__global__ void __launch_bounds__(kLpInThreads)
+    lpips_max_pool3s2_kernel(const float* __restrict__ f, int N, int H, int W, int C, int OH, int OW, float* __restrict__ out) {
+  const int cq = C / 4;
+  const int n = OH * OW * cq;
+  const int i = blockIdx.x * kLpInThreads + threadIdx.x;
+  if (i >= n) return;
+  const int q = i % cq, pos = i / cq;
+  const int oh = pos / OW, ow = pos % OW;
+  for (int img = blockIdx.y; img < N; img += gridDim.y) {
+    const float4* src = reinterpret_cast<const float4*>(f + static_cast<long long>(img) * H * W * C) + q;
+    float4 m = make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);
+#pragma unroll
+    for (int kh = 0; kh < 3; ++kh)
+#pragma unroll
+      for (int kw = 0; kw < 3; ++kw) {
+        const float4 v = __ldg(src + (static_cast<long long>(2 * oh + kh) * W + 2 * ow + kw) * cq);
+        m = make_float4(fmaxf(m.x, v.x), fmaxf(m.y, v.y), fmaxf(m.z, v.z), fmaxf(m.w, v.w));
+      }
+    reinterpret_cast<float4*>(out + static_cast<long long>(img) * n * 4)[i] =
+        make_float4(tf32_rn(m.x), tf32_rn(m.y), tf32_rn(m.z), tf32_rn(m.w));
+  }
+}
+
+// The 5 x 5 taps (zero padding 2) of x [N, H, W, C] packed into channels, so that AlexNet's conv2 runs as a 1 x 1
+// convolution: out [N, H, W, 25 C], channel (kh * 5 + kw) * C + c of position (h, w) is x(h + kh - 2, w + kw - 2, c), 0
+// outside the image.  An exact copy.  One thread per four channels of an output position.
+__global__ void __launch_bounds__(kLpInThreads)
+    lpips_pack5x5_kernel(const float* __restrict__ x, int N, int H, int W, int C, float* __restrict__ out) {
+  const int cq = C / 4, oq = 25 * cq;
+  const int n = H * W * oq;
+  const int i = blockIdx.x * kLpInThreads + threadIdx.x;
+  if (i >= n) return;
+  const int q = i % oq, pos = i / oq;
+  const int tap = q / cq, c4 = q % cq;
+  const int y = pos / W + tap / 5 - 2, xw = pos % W + tap % 5 - 2;
+  const bool in = y >= 0 && y < H && xw >= 0 && xw < W;
+  for (int img = blockIdx.y; img < N; img += gridDim.y) {
+    const float4* src = reinterpret_cast<const float4*>(x + static_cast<long long>(img) * H * W * C);
+    reinterpret_cast<float4*>(out + static_cast<long long>(img) * n * 4)[i] =
+        in ? __ldg(src + (static_cast<long long>(y) * W + xw) * cq + c4) : make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+}
+
 // kV consecutive channels of one position, lane l holding [l*kV, l*kV + kV)
 template <int kV>
 __device__ __forceinline__ void lp_load(const float* p, float (&v)[kV]) {
@@ -82,6 +169,13 @@ __device__ __forceinline__ void lp_load(const float* p, float (&v)[kV]) {
     const float2 q = __ldg(reinterpret_cast<const float2*>(p));
     v[0] = q.x;
     v[1] = q.y;
+  } else if constexpr (kV % 4 == 2) {   // C = 192: 24 bytes per lane, 8-byte aligned
+#pragma unroll
+    for (int i = 0; i < kV / 2; ++i) {
+      const float2 q = __ldg(reinterpret_cast<const float2*>(p) + i);
+      v[2 * i] = q.x;
+      v[2 * i + 1] = q.y;
+    }
   } else {
 #pragma unroll
     for (int i = 0; i < kV / 4; ++i) {
@@ -97,6 +191,9 @@ template <int kV>
 __device__ __forceinline__ void lp_store(float* p, const float (&v)[kV]) {
   if constexpr (kV == 2) {
     *reinterpret_cast<float2*>(p) = make_float2(v[0], v[1]);
+  } else if constexpr (kV % 4 == 2) {
+#pragma unroll
+    for (int i = 0; i < kV / 2; ++i) reinterpret_cast<float2*>(p)[i] = make_float2(v[2 * i], v[2 * i + 1]);
   } else {
 #pragma unroll
     for (int i = 0; i < kV / 4; ++i)
@@ -114,11 +211,11 @@ __device__ __forceinline__ double warp_sum(double v) {
 // of the normalised features, in units of 2^-32.  pooled (optional) [2T, H/2, W/2, C]: 2 x 2 max pool, floor, rounded to
 // TF32 (rounding is monotonic, so this is the rounded max of the four values).
 // CTA (t, blk) owns quads [blk * 32, blk * 32 + 32) of frame t in row-major quad order; warp w of it quads 4w .. 4w + 3.
-// Two CTAs per SM at least below C = 512: left to itself ptxas gives C = 64 / 128 48 / 64 registers and spills.
-template <int C>
-__global__ void __launch_bounds__(kLpTapThreads, C >= 512 ? 1 : 2)
-    lpips_tap_kernel(const float* __restrict__ f, int T, int H, int W, const float* __restrict__ lin_w,
-                     unsigned long long* __restrict__ acc, float* __restrict__ pooled, int ctas_per_frame) {
+// kCopy: `pooled` is instead `copy` [2T, H, W, C], which receives every position of f rounded to the nearest TF32 value
+// (a tap whose next consumer is a convolution, AlexNet's relu3 and relu4); there is no pool.
+template <int C, bool kCopy>
+__device__ __forceinline__ void lpips_tap(const float* __restrict__ f, int T, int H, int W, const float* __restrict__ lin_w,
+                                          unsigned long long* __restrict__ acc, float* __restrict__ pooled, int ctas_per_frame) {
   constexpr int kV = C / 32;
   __shared__ double s_red[kLpTapThreads / 32];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -151,6 +248,16 @@ __global__ void __launch_bounds__(kLpTapThreads, C >= 512 ? 1 : 2)
       float va[kV], vb[kV];
       lp_load<kV>(fa + off, va);
       lp_load<kV>(fb + off, vb);
+      if constexpr (kCopy) {
+        float ra[kV], rb[kV];
+#pragma unroll
+        for (int k = 0; k < kV; ++k) {
+          ra[k] = tf32_rn(va[k]);
+          rb[k] = tf32_rn(vb[k]);
+        }
+        lp_store<kV>(pooled + (fa - f) + off, ra);
+        lp_store<kV>(pooled + (fb - f) + off, rb);
+      }
       double sa = 0.0, sb = 0.0;
 #pragma unroll
       for (int k = 0; k < kV; ++k) {
@@ -169,7 +276,7 @@ __global__ void __launch_bounds__(kLpTapThreads, C >= 512 ? 1 : 2)
         mb[k] = fmaxf(mb[k], vb[k]);
       }
     }
-    if (pooled && full) {
+    if (!kCopy && pooled && full) {
       const long long po = (static_cast<long long>(qh) * PW + qw) * C + lane * kV;
       const long long pstride = static_cast<long long>(PH) * PW * C;
 #pragma unroll
@@ -190,6 +297,70 @@ __global__ void __launch_bounds__(kLpTapThreads, C >= 512 ? 1 : 2)
     for (int i = 0; i < kLpTapThreads / 32; ++i) s += s_red[i];
     atomicAdd(acc + t, static_cast<unsigned long long>(__double2ll_rn(s * 4294967296.0)));
   }
+}
+
+// Two CTAs per SM at least below C = 384: left to itself ptxas gives C = 64 / 128 48 / 64 registers and spills.
+template <int C>
+__global__ void __launch_bounds__(kLpTapThreads, C >= 384 ? 1 : 2)
+    lpips_tap_kernel(const float* __restrict__ f, int T, int H, int W, const float* __restrict__ lin_w,
+                     unsigned long long* __restrict__ acc, float* __restrict__ pooled, int ctas_per_frame) {
+  lpips_tap<C, false>(f, T, H, W, lin_w, acc, pooled, ctas_per_frame);
+}
+template <int C>
+__global__ void __launch_bounds__(kLpTapThreads, C >= 384 ? 1 : 2)
+    lpips_tap_copy_kernel(const float* __restrict__ f, int T, int H, int W, const float* __restrict__ lin_w,
+                          unsigned long long* __restrict__ acc, float* __restrict__ copy, int ctas_per_frame) {
+  lpips_tap<C, true>(f, T, H, W, lin_w, acc, copy, ctas_per_frame);
+}
+
+// y extent of the pixel kernels' grids: images are walked along y, 32-bit indices within an image along x
+inline dim3 lp_image_grid(int per_image, long long images) {
+  return dim3(static_cast<unsigned>((per_image + kLpInThreads - 1) / kLpInThreads),
+              static_cast<unsigned>(images < 65535 ? images : 65535));
+}
+
+// the checks and launch shared by cvvae_lpips_tap (pooled: NULL or the 2 x 2 pool) and cvvae_lpips_tap_copy
+template <bool kCopy>
+int lpips_tap_launch(const char* who, const float* f, int32_t T, int32_t H, int32_t W, int32_t C, const float* lin_w,
+                     int64_t* acc, float* pooled, void* stream_) {
+  const char* side = kCopy ? "copy" : "pooled";
+  CVVAE_CHECK_ARG(f && lin_w && acc && (!kCopy || pooled), "%s: null pointer", who);
+  if (kCopy)
+    CVVAE_CHECK_ARG(C == 256 || C == 384, "%s: C must be 256 or 384, got %d", who, (int)C);
+  else
+    CVVAE_CHECK_ARG(C == 64 || C == 128 || C == 192 || C == 256 || C == 384 || C == 512,
+                    "%s: C must be 64, 128, 192, 256, 384 or 512, got %d", who, (int)C);
+  CVVAE_CHECK_ARG(T >= 0 && H >= 1 && W >= 1, "%s: needs T >= 0 and H, W >= 1, got T=%d H=%d W=%d", who, (int)T, (int)H,
+                  (int)W);
+  CVVAE_CHECK_ARG(kCopy || !pooled || (H >= 2 && W >= 2), "%s: pooling needs H, W >= 2, got %d x %d", who, (int)H, (int)W);
+  CVVAE_CHECK_ARG(1ll * H * W <= kLpMaxPositions,
+                  "%s: %d x %d positions exceed the 64-bit accumulator's range (H*W <= 2^23)", who, (int)H, (int)W);
+  CVVAE_CHECK_ARG(reinterpret_cast<uintptr_t>(f) % 16 == 0 && reinterpret_cast<uintptr_t>(lin_w) % 16 == 0 &&
+                      reinterpret_cast<uintptr_t>(pooled) % 16 == 0,
+                  "%s: f, lin_w and %s must be 16-byte aligned", who, side);
+  if (T == 0) return CVVAE_OK;
+  const long long quads = 1ll * ((H + 1) / 2) * ((W + 1) / 2);
+  const long long per_frame = (quads + kLpQuadsPerCta - 1) / kLpQuadsPerCta;
+  const long long grid = per_frame * T;
+  CVVAE_CHECK_ARG(grid < (1ll << 31), "%s: too many frames for one launch (T=%d at %d x %d)", who, (int)T, (int)H, (int)W);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  CVVAE_CUDA(cudaMemsetAsync(acc, 0, sizeof(int64_t) * T, stream));
+  unsigned long long* out = reinterpret_cast<unsigned long long*>(acc);
+  const unsigned g = static_cast<unsigned>(grid);
+  const int pf = static_cast<int>(per_frame);
+  if constexpr (kCopy) {
+    if (C == 256) lpips_tap_copy_kernel<256><<<g, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, out, pooled, pf);
+    else lpips_tap_copy_kernel<384><<<g, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, out, pooled, pf);
+  } else {
+    if (C == 64) lpips_tap_kernel<64><<<g, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, out, pooled, pf);
+    else if (C == 128) lpips_tap_kernel<128><<<g, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, out, pooled, pf);
+    else if (C == 192) lpips_tap_kernel<192><<<g, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, out, pooled, pf);
+    else if (C == 256) lpips_tap_kernel<256><<<g, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, out, pooled, pf);
+    else if (C == 384) lpips_tap_kernel<384><<<g, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, out, pooled, pf);
+    else lpips_tap_kernel<512><<<g, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, out, pooled, pf);
+  }
+  CVVAE_LAUNCH_CHECK();
+  return CVVAE_OK;
 }
 
 }  // namespace cvvae
@@ -213,31 +384,60 @@ extern "C" int cvvae_lpips_input(const uint8_t* a_thwc, const uint8_t* b_thwc, i
 }
 
 extern "C" int cvvae_lpips_tap(const float* f, int32_t T, int32_t H, int32_t W, int32_t C, const float* lin_w, int64_t* acc,
-                               float* pooled, void* stream_) {
-  CVVAE_CHECK_ARG(f && lin_w && acc, "cvvae_lpips_tap: null pointer");
-  CVVAE_CHECK_ARG(C == 64 || C == 128 || C == 256 || C == 512, "cvvae_lpips_tap: C must be 64, 128, 256 or 512, got %d", (int)C);
-  CVVAE_CHECK_ARG(T >= 0 && H >= 1 && W >= 1, "cvvae_lpips_tap: needs T >= 0 and H, W >= 1, got T=%d H=%d W=%d", (int)T, (int)H,
-                  (int)W);
-  CVVAE_CHECK_ARG(!pooled || (H >= 2 && W >= 2), "cvvae_lpips_tap: pooling needs H, W >= 2, got %d x %d", (int)H, (int)W);
-  CVVAE_CHECK_ARG(1ll * H * W <= kLpMaxPositions,
-                  "cvvae_lpips_tap: %d x %d positions exceed the 64-bit accumulator's range (H*W <= 2^23)", (int)H, (int)W);
-  CVVAE_CHECK_ARG(reinterpret_cast<uintptr_t>(f) % 16 == 0 && reinterpret_cast<uintptr_t>(lin_w) % 16 == 0 &&
-                      reinterpret_cast<uintptr_t>(pooled) % 16 == 0,
-                  "cvvae_lpips_tap: f, lin_w and pooled must be 16-byte aligned");
+                               float* pooled, void* stream) {
+  return lpips_tap_launch<false>("cvvae_lpips_tap", f, T, H, W, C, lin_w, acc, pooled, stream);
+}
+
+extern "C" int cvvae_lpips_tap_copy(const float* f, int32_t T, int32_t H, int32_t W, int32_t C, const float* lin_w,
+                                    int64_t* acc, float* copy, void* stream) {
+  return lpips_tap_launch<true>("cvvae_lpips_tap_copy", f, T, H, W, C, lin_w, acc, copy, stream);
+}
+
+extern "C" int cvvae_lpips_alex_input(const uint8_t* a_thwc, const uint8_t* b_thwc, int32_t T, int32_t H, int32_t W, float* out,
+                                      void* stream) {
+  CVVAE_CHECK_ARG(a_thwc && b_thwc && out, "cvvae_lpips_alex_input: null pointer");
+  CVVAE_CHECK_ARG(T >= 0 && H >= 7 && W >= 7, "cvvae_lpips_alex_input: needs T >= 0 and H, W >= 7, got T=%d H=%d W=%d",
+                  (int)T, (int)H, (int)W);
+  CVVAE_CHECK_ARG(reinterpret_cast<uintptr_t>(out) % 16 == 0, "cvvae_lpips_alex_input: `out` must be 16-byte aligned");
+  const int OH = (H - 7) / 4 + 1, OW = (W - 7) / 4 + 1;
+  CVVAE_CHECK_ARG(1ll * OH * OW * (kLpAlexInChannels / 4) < (1ll << 31),
+                  "cvvae_lpips_alex_input: %d x %d frames are too large for one launch", (int)H, (int)W);
   if (T == 0) return CVVAE_OK;
-  const long long quads = 1ll * ((H + 1) / 2) * ((W + 1) / 2);
-  const long long per_frame = (quads + kLpQuadsPerCta - 1) / kLpQuadsPerCta;
-  const long long grid = per_frame * T;
-  CVVAE_CHECK_ARG(grid < (1ll << 31), "cvvae_lpips_tap: too many frames for one launch (T=%d at %d x %d)", (int)T, (int)H, (int)W);
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  CVVAE_CUDA(cudaMemsetAsync(acc, 0, sizeof(int64_t) * T, stream));
-  unsigned long long* out = reinterpret_cast<unsigned long long*>(acc);
-  const unsigned g = static_cast<unsigned>(grid);
-  const int pf = static_cast<int>(per_frame);
-  if (C == 64) lpips_tap_kernel<64><<<g, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, out, pooled, pf);
-  else if (C == 128) lpips_tap_kernel<128><<<g, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, out, pooled, pf);
-  else if (C == 256) lpips_tap_kernel<256><<<g, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, out, pooled, pf);
-  else lpips_tap_kernel<512><<<g, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, out, pooled, pf);
+  lpips_alex_input_kernel<<<lp_image_grid(OH * OW * (kLpAlexInChannels / 4), 2ll * T), kLpInThreads, 0,
+                            static_cast<cudaStream_t>(stream)>>>(a_thwc, b_thwc, T, H, W, OH, OW, out);
+  CVVAE_LAUNCH_CHECK();
+  return CVVAE_OK;
+}
+
+extern "C" int cvvae_lpips_max_pool3s2(const float* f, int32_t N, int32_t H, int32_t W, int32_t C, float* out, void* stream) {
+  CVVAE_CHECK_ARG(f && out, "cvvae_lpips_max_pool3s2: null pointer");
+  CVVAE_CHECK_ARG(N >= 0 && H >= 3 && W >= 3 && C >= 4 && C % 4 == 0,
+                  "cvvae_lpips_max_pool3s2: needs N >= 0, H, W >= 3 and C a positive multiple of 4, got N=%d H=%d W=%d C=%d",
+                  (int)N, (int)H, (int)W, (int)C);
+  CVVAE_CHECK_ARG(reinterpret_cast<uintptr_t>(f) % 16 == 0 && reinterpret_cast<uintptr_t>(out) % 16 == 0,
+                  "cvvae_lpips_max_pool3s2: f and out must be 16-byte aligned");
+  const int OH = (H - 3) / 2 + 1, OW = (W - 3) / 2 + 1;
+  CVVAE_CHECK_ARG(1ll * H * W * C < (1ll << 31), "cvvae_lpips_max_pool3s2: %d x %d x %d is too large for one launch", (int)H,
+                  (int)W, (int)C);
+  if (N == 0) return CVVAE_OK;
+  lpips_max_pool3s2_kernel<<<lp_image_grid(OH * OW * (C / 4), N), kLpInThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+      f, N, H, W, C, OH, OW, out);
+  CVVAE_LAUNCH_CHECK();
+  return CVVAE_OK;
+}
+
+extern "C" int cvvae_lpips_pack5x5(const float* x, int32_t N, int32_t H, int32_t W, int32_t C, float* out, void* stream) {
+  CVVAE_CHECK_ARG(x && out, "cvvae_lpips_pack5x5: null pointer");
+  CVVAE_CHECK_ARG(N >= 0 && H >= 1 && W >= 1 && C >= 4 && C % 4 == 0,
+                  "cvvae_lpips_pack5x5: needs N >= 0, H, W >= 1 and C a positive multiple of 4, got N=%d H=%d W=%d C=%d",
+                  (int)N, (int)H, (int)W, (int)C);
+  CVVAE_CHECK_ARG(reinterpret_cast<uintptr_t>(x) % 16 == 0 && reinterpret_cast<uintptr_t>(out) % 16 == 0,
+                  "cvvae_lpips_pack5x5: x and out must be 16-byte aligned");
+  CVVAE_CHECK_ARG(25ll * H * W * C < (1ll << 31), "cvvae_lpips_pack5x5: %d x %d x %d is too large for one launch", (int)H,
+                  (int)W, (int)C);
+  if (N == 0) return CVVAE_OK;
+  lpips_pack5x5_kernel<<<lp_image_grid(H * W * 25 * (C / 4), N), kLpInThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+      x, N, H, W, C, out);
   CVVAE_LAUNCH_CHECK();
   return CVVAE_OK;
 }

@@ -43,6 +43,15 @@ point, so results are bit-reproducible, independent of how frames are grouped, e
 symmetric in a and b.  Frames need at least 16 x 16 px (relu5_3 is H/16 x W/16) and at most 2^23 px (the range of the
 fixed-point sums).  No weights ship with the package:
 ``LPIPS.from_state_dict`` takes torchvision's VGG16 state dict (or the reference module's) and the lpips heads.
+
+``LPIPS.from_state_dict(..., net="alex")`` is the same metric on AlexNet features, the lpips package's default network
+(``lpips.LPIPS()``, and the LPIPS column of most published reconstruction tables; the two networks give different
+numbers).  Only the trunk differs: torchvision's ``alexnet().features[0:12]``, i.e. conv1 (11 x 11, stride 4, padding 2)
+-> relu1, a 3 x 3 stride-2 max pool (floor), conv2 (5 x 5, padding 2) -> relu2, the same pool, conv3 .. conv5 (3 x 3,
+padding 1) -> relu3 .. relu5, with C = 64, 192, 384, 256, 256 at the taps (``features[12]``, the last pool, is not
+part of LPIPS).  conv1 and conv2 run as 1 x 1 tensor-core convolutions over their taps packed into channels; the taps
+are h1 = (H - 7) // 4 + 1, p1 = (h1 - 3) // 2 + 1 for relu2, p2 = (p1 - 3) // 2 + 1 for relu3 .. relu5 (likewise W), so
+frames need at least 31 x 31 px.  The ``spatial=True`` variant (maps upsampled to the input size) is not provided.
 """
 from __future__ import annotations
 
@@ -66,6 +75,13 @@ LPIPS_MAX_HEAD = 32.0         # |w| bound of the heads that keeps the tap kernel
 # vgg16.features indices of the thirteen convolutions, per block (the reference's slice1 .. slice5); each block ends in a tap
 _VGG_BLOCKS = ((0, 2), (5, 7), (10, 12, 14), (17, 19, 21), (24, 26, 28))
 _VGG_CHANNELS = (64, 128, 256, 512, 512)
+LPIPS_NETS = ("vgg", "alex")
+LPIPS_ALEX_MIN_SIZE = 31      # AlexNet: relu3 .. relu5 have (p1 - 3) // 2 + 1 >= 1 rows, p1 = ((H - 7) // 4 - 2) // 2 + 1
+LPIPS_ALEX_LAUNCHES = 14      # per group of frames: the input kernel, 5 convolutions, 5 taps, 2 pools, conv2's packing
+# alexnet.features index, Cin, kernel extent of the five convolutions (lpips' slice1 .. slice5 hold one each), and the taps
+_ALEX_CONVS = ((0, 3, 11), (3, 64, 5), (6, 192, 3), (8, 384, 3), (10, 256, 3))
+_ALEX_CHANNELS = (64, 192, 384, 256, 256)
+_ALEX_IN_CHANNELS = 384       # conv1's 3 x 11 x 11 = 363 taps, padded to a multiple of the channel block
 
 
 class FrameMetrics(NamedTuple):
@@ -163,7 +179,11 @@ def frame_ms_ssim(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
     return _ms_ssim_scores(_launch_ms_ssim(a.contiguous(), b.contiguous()).cpu(), H, W)
 
 
-def _check_lpips_size(H: int, W: int, who: str) -> None:
+def _check_lpips_size(H: int, W: int, who: str, net: str = "vgg") -> None:
+    if net == "alex" and min(H, W) < LPIPS_ALEX_MIN_SIZE:
+        raise ValueError(f"{who}: LPIPS (AlexNet) needs frames of at least {LPIPS_ALEX_MIN_SIZE} x {LPIPS_ALEX_MIN_SIZE} px "
+                         f"(its last taps, relu3 .. relu5, follow the stride-4 conv1 and two 3 x 3 stride-2 pools); got "
+                         f"{H} x {W}")
     if min(H, W) < LPIPS_MIN_SIZE:
         raise ValueError(f"{who}: LPIPS needs frames of at least {LPIPS_MIN_SIZE} x {LPIPS_MIN_SIZE} px (its last tap, "
                          f"relu5_3, is 1/16 of the size); got {H} x {W}")
@@ -176,17 +196,28 @@ def _lpips_tap_sizes(H: int, W: int) -> list:
     return [(H >> k, W >> k) for k in range(len(_VGG_BLOCKS))]
 
 
-def _lpips_scores(acc: torch.Tensor, H: int, W: int) -> torch.Tensor:
+def _lpips_alex_tap_sizes(H: int, W: int) -> list:
+    """(h, w) of AlexNet's five taps: relu1 after conv1 (11 x 11, stride 4, padding 2), relu2 after a 3 x 3 stride-2 max
+    pool (floor) and the 'same' conv2, relu3 .. relu5 after a second such pool and 'same' 3 x 3 convolutions."""
+    def sizes(n: int) -> tuple:
+        c1 = (n - 7) // 4 + 1
+        p1 = (c1 - 3) // 2 + 1
+        return c1, p1, (p1 - 3) // 2 + 1
+    (h1, hp1, hp2), (w1, wp1, wp2) = sizes(H), sizes(W)
+    return [(h1, w1), (hp1, wp1)] + [(hp2, wp2)] * 3
+
+
+def _lpips_scores(acc: torch.Tensor, H: int, W: int, net: str = "vgg") -> torch.Tensor:
     """Host int64 [5, T] of the tap kernels (per tap and frame, the sum over positions times 2^32) -> LPIPS, float64 [T]."""
     d = torch.zeros(acc.shape[1], dtype=torch.float64)
-    for k, (h, w) in enumerate(_lpips_tap_sizes(H, W)):
+    for k, (h, w) in enumerate(_lpips_alex_tap_sizes(H, W) if net == "alex" else _lpips_tap_sizes(H, W)):
         d += acc[k].double() / 4294967296.0 / (h * w)
     return d
 
 
-def _lpips_weights(state_dicts: tuple) -> tuple:
-    """The checked weights of ``LPIPS.from_state_dict`` on the host, fp32: ([(weight, bias)] of the thirteen
-    convolutions, [head [C_k]] of the five taps)."""
+def _lpips_weights(state_dicts: tuple, net: str = "vgg") -> tuple:
+    """The checked weights of ``LPIPS.from_state_dict`` on the host, fp32: ([(weight, bias)] of the convolutions
+    (VGG16: thirteen, AlexNet: five), [head [C_k]] of the five taps)."""
     sd: dict = {}
     for d in state_dicts:
         sd.update(d)
@@ -213,15 +244,21 @@ def _lpips_weights(state_dicts: tuple) -> tuple:
             v = get((key,), (1, 3, 1, 1))
             if not torch.equal(v.flatten(), torch.tensor(want, dtype=torch.float32)):
                 raise ValueError(f"LPIPS.from_state_dict: {key!r} is {v.flatten().tolist()}, expected {list(want)}")
+    # per convolution: lpips slice k (0-based), features index i, Cin, Cout, kernel extent
+    if net == "alex":
+        layers = [(k, i, cin, c, ks) for k, ((i, cin, ks), c) in enumerate(zip(_ALEX_CONVS, _ALEX_CHANNELS))]
+    else:
+        layers, cin = [], 3
+        for k, (block, c) in enumerate(zip(_VGG_BLOCKS, _VGG_CHANNELS)):
+            for i in block:
+                layers.append((k, i, cin, c, 3))
+                cin = c
     convs = []
-    cin = 3
-    for k, (block, c) in enumerate(zip(_VGG_BLOCKS, _VGG_CHANNELS)):
-        for i in block:
-            keys = lambda s: (f"features.{i}.{s}", f"net.slice{k + 1}.{i}.{s}")   # noqa: E731
-            convs.append((get(keys("weight"), (c, cin, 3, 3)), get(keys("bias"), (c,))))
-            cin = c
+    for k, i, cin, c, ks in layers:
+        keys = lambda s: (f"features.{i}.{s}", f"net.slice{k + 1}.{i}.{s}")   # noqa: E731
+        convs.append((get(keys("weight"), (c, cin, ks, ks)), get(keys("bias"), (c,))))
     heads = []
-    for k, c in enumerate(_VGG_CHANNELS):
+    for k, c in enumerate(_ALEX_CHANNELS if net == "alex" else _VGG_CHANNELS):
         key = f"lin{k}.model.1.weight"
         v = get((key,), (1, c, 1, 1))
         if v.abs().max().item() > LPIPS_MAX_HEAD:
@@ -233,32 +270,50 @@ def _lpips_weights(state_dicts: tuple) -> tuple:
 
 
 class LPIPS:
-    """LPIPS (VGG16, lpips v0.1) of every frame of `b` against the same frame of `a` on the GPU; the module docstring has
-    the definition.  Build it with ``LPIPS.from_state_dict``; ``metric(a, b)`` takes two CUDA uint8 ``[T, H, W, 3]``
-    videos on ``metric.device`` (H, W >= 16, H * W <= 2^23) and returns float64 ``[T]`` on the host.
+    """LPIPS (lpips v0.1, VGG16 or AlexNet features) of every frame of `b` against the same frame of `a` on the GPU; the
+    module docstring has the definition.  Build it with ``LPIPS.from_state_dict``; ``metric(a, b)`` takes two CUDA uint8
+    ``[T, H, W, 3]`` videos on ``metric.device`` (H, W >= ``metric.min_size``, H * W <= 2^23) and returns float64 ``[T]``
+    on the host.  ``metric.net`` is ``"vgg"`` or ``"alex"``.
 
-    Frames are scored in groups whose VGG activations stay within ``LPIPS_GROUP_BYTES``; each group is
-    ``LPIPS_LAUNCHES`` kernel launches on the current stream of the device.  The result is the same, bit for bit,
-    whatever the grouping."""
+    Frames are scored in groups whose activations stay within ``LPIPS_GROUP_BYTES``; each group is ``metric.launches``
+    kernel launches on the current stream of the device.  The result is the same, bit for bit, whatever the grouping."""
 
-    def __init__(self, blocks: list, heads: list, device: torch.device):
+    net = "vgg"   # the network of an instance built without naming one
+
+    def __init__(self, blocks: list, heads: list, device: torch.device, net: str = "vgg"):
         from .ops import CudaOps
         self._ops = CudaOps()
         self._blocks = blocks          # per block: [(packed weight, bias, 1 x 1 tap-packed?)]
         self._heads = heads            # fp32 [C_k] per tap
         self.device = device
+        self.net = net
         self._group_bytes = LPIPS_GROUP_BYTES
 
+    @property
+    def min_size(self) -> int:
+        """The smallest frame side the network accepts: 16 px for VGG16, 31 px for AlexNet."""
+        return LPIPS_ALEX_MIN_SIZE if self.net == "alex" else LPIPS_MIN_SIZE
+
+    @property
+    def launches(self) -> int:
+        """Kernel launches per group of frames."""
+        return LPIPS_ALEX_LAUNCHES if self.net == "alex" else LPIPS_LAUNCHES
+
     @classmethod
-    def from_state_dict(cls, *state_dicts, device=None) -> "LPIPS":
-        """Weights from one or more state dicts, merged (later ones win): the thirteen convolutions under torchvision's
-        keys ``features.{i}.weight`` / ``.bias`` (``vgg16-397923af.pth``) or the reference module's ``net.slice{k}.{i}.*``
-        (same i), the heads under ``lin{k}.model.1.weight`` ``[1, C_k, 1, 1]`` (lpips v0.1 ``vgg.pth``, or the reference's
-        ``LPIPS().state_dict()``).  ``scaling_layer.shift`` / ``.scale``, if present, must be the constants above; every
-        other key is ignored.  A missing key, a wrong shape, a non-float or non-finite value, or a head with |w| > 32
-        raises ValueError.  `device`: a CUDA device (default: the current one).  The weights are packed once, the
-        convolutions' rounded to TF32."""
-        convs, heads = _lpips_weights(state_dicts)
+    def from_state_dict(cls, *state_dicts, device=None, net: str = "vgg") -> "LPIPS":
+        """Weights from one or more state dicts, merged (later ones win).  ``net="vgg"`` (the default): the thirteen
+        convolutions under torchvision's keys ``features.{i}.weight`` / ``.bias`` (``vgg16-397923af.pth``) or the
+        reference module's ``net.slice{k}.{i}.*`` (same i), the heads under ``lin{k}.model.1.weight`` ``[1, C_k, 1, 1]``
+        (lpips v0.1 ``vgg.pth``, or the reference's ``LPIPS().state_dict()``).  ``net="alex"``, the lpips package's
+        default network: the five convolutions ``features.{0,3,6,8,10}.*`` of torchvision's AlexNet
+        (``alexnet-owt-7be5be79.pth``) or the lpips module's ``net.slice{k}.{i}.*``, and the heads of lpips v0.1
+        ``alex.pth`` (C_k = 64, 192, 384, 256, 256).  ``scaling_layer.shift`` / ``.scale``, if present, must be the
+        constants above; every other key is ignored.  A missing key, a wrong shape, a non-float or non-finite value, a
+        head with |w| > 32 or an unknown `net` raises ValueError.  `device`: a CUDA device (default: the current one).
+        The weights are packed once, the convolutions' rounded to TF32."""
+        if net not in LPIPS_NETS:
+            raise ValueError(f"LPIPS.from_state_dict: `net` must be one of {LPIPS_NETS}, got {net!r}")
+        convs, heads = _lpips_weights(state_dicts, net)
         dev = torch.device(device) if device is not None else None
         if dev is not None and dev.type != "cuda":
             raise ValueError(f"LPIPS.from_state_dict: the device must be a CUDA device, got {dev}")
@@ -266,6 +321,8 @@ class LPIPS:
             dev = torch.device("cuda", torch.cuda.current_device() if dev is None or dev.index is None else dev.index)
         from .ops import CudaOps
         ops = CudaOps()
+        if net == "alex":
+            return cls(_alex_blocks(ops, convs, dev), [h.to(dev) for h in heads], dev, net)
         blocks, n = [], 0
         for k, block in enumerate(_VGG_BLOCKS):
             layers = []
@@ -282,8 +339,12 @@ class LPIPS:
         return m
 
     def _group(self, H: int, W: int) -> int:
-        """Frames per group: the largest activations live at once are conv1_2's input and output, 64 + 64 fp32 channels
-        at full size for both videos."""
+        """Frames per group.  VGG16: the largest activations live at once are conv1_2's input and output, 64 + 64 fp32
+        channels at full size for both videos.  AlexNet: conv1's packed input and output (384 + 64 channels) or conv2's
+        (1600 + 192), whichever is larger."""
+        if self.net == "alex":
+            (h1, w1), (h2, w2) = _lpips_alex_tap_sizes(H, W)[:2]
+            return max(1, self._group_bytes // (2 * 4 * max((_ALEX_IN_CHANNELS + 64) * h1 * w1, (1600 + 192) * h2 * w2)))
         return max(1, self._group_bytes // (2 * 128 * 4 * H * W))
 
     @L._on_tensor_device
@@ -298,6 +359,8 @@ class LPIPS:
         return acc
 
     def _run_group(self, a: torch.Tensor, b: torch.Tensor, acc: torch.Tensor) -> None:
+        if self.net == "alex":
+            return self._run_group_alex(a, b, acc)
         G, H, W, _ = a.shape
         lib, dev, stream = self._ops.lib, a.device, L._stream(a)
         x = torch.empty((2 * G, 1, H, W, 32), dtype=torch.float32, device=dev)
@@ -322,12 +385,78 @@ class LPIPS:
             if pooled is not None:
                 x, h, w = pooled, h // 2, w // 2
 
+    def _run_group_alex(self, a: torch.Tensor, b: torch.Tensor, acc: torch.Tensor) -> None:
+        """AlexNet's features[0:12] on both videos, every convolution output a tap (fp32); what only a convolution reads
+        is TF32: conv1's packed input, the pools (hence conv2's packed input) and the copies of relu3 and relu4."""
+        G, H, W, _ = a.shape
+        lib, dev, stream = self._ops.lib, a.device, L._stream(a)
+        sizes = _lpips_alex_tap_sizes(H, W)
+        convs = [block[0][:2] for block in self._blocks]   # (packed weight, bias) of conv1 .. conv5
+
+        def conv(x, wp, bias, k, three_by_three):
+            y = torch.empty((2 * G, 1, *sizes[k], wp.shape[1]), dtype=torch.float32, device=dev)
+            if three_by_three:
+                return self._ops.conv(x, wp, bias, kernel=(1, 3, 3), offset=(0, -1, -1), out=y, relu=True)
+            return self._ops.conv(x, wp, bias, out=y, relu=True)
+
+        def tap(f, k, copy=None):
+            h, w = sizes[k]
+            args = (f.data_ptr(), G, h, w, f.shape[-1], self._heads[k].data_ptr(), acc[k].data_ptr())
+            if copy is None:
+                L.check(lib.cvvae_lpips_tap(*args, None, stream), "cvvae_lpips_tap")
+            else:
+                L.check(lib.cvvae_lpips_tap_copy(*args, copy.data_ptr(), stream), "cvvae_lpips_tap_copy")
+
+        def pool(f, k):
+            (h, w), (oh, ow) = sizes[k], sizes[k + 1]
+            out = torch.empty((2 * G, 1, oh, ow, f.shape[-1]), dtype=torch.float32, device=dev)
+            L.check(lib.cvvae_lpips_max_pool3s2(f.data_ptr(), 2 * G, h, w, f.shape[-1], out.data_ptr(), stream),
+                    "cvvae_lpips_max_pool3s2")
+            return out
+
+        x = torch.empty((2 * G, 1, *sizes[0], _ALEX_IN_CHANNELS), dtype=torch.float32, device=dev)
+        L.check(lib.cvvae_lpips_alex_input(a.data_ptr(), b.data_ptr(), G, H, W, x.data_ptr(), stream),
+                "cvvae_lpips_alex_input")
+        f = conv(x, *convs[0], 0, False)
+        del x
+        tap(f, 0)
+        p = pool(f, 0)
+        del f
+        x = torch.empty((2 * G, 1, *sizes[1], 25 * p.shape[-1]), dtype=torch.float32, device=dev)
+        L.check(lib.cvvae_lpips_pack5x5(p.data_ptr(), 2 * G, *sizes[1], p.shape[-1], x.data_ptr(), stream),
+                "cvvae_lpips_pack5x5")
+        del p
+        f = conv(x, *convs[1], 1, False)
+        del x
+        tap(f, 1)
+        x = pool(f, 1)
+        for k in (2, 3, 4):
+            f = conv(x, *convs[k], k, True)
+            x = torch.empty_like(f) if k < 4 else None   # relu3 and relu4 feed the next convolution: their TF32 copy
+            tap(f, k, x)
+
     def __call__(self, a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
         _check_frames(a, b, "LPIPS")
         if a.device != self.device:
             raise ValueError(f"LPIPS: the frames are on {a.device}, the weights on {self.device}")
         T, H, W, _ = a.shape
-        _check_lpips_size(H, W, "LPIPS")
+        _check_lpips_size(H, W, "LPIPS", self.net)
         if T == 0:
             return torch.empty(0, dtype=torch.float64)
-        return _lpips_scores(self._launch(a.contiguous(), b.contiguous()).cpu(), H, W)
+        return _lpips_scores(self._launch(a.contiguous(), b.contiguous()).cpu(), H, W, self.net)
+
+
+def _alex_blocks(ops, convs: list, dev: torch.device) -> list:
+    """AlexNet's five convolutions packed for conv_tc, one per block ([(packed weight, bias, 1 x 1 tap-packed?)]):
+    conv1 as a 1 x 1 convolution over the 384 channels of cvvae_lpips_alex_input ((c, kh, kw) order, zero-padded),
+    conv2 as one over the 1600 of cvvae_lpips_pack5x5 ((kh, kw, c) order), conv3 .. conv5 as 3 x 3 convolutions."""
+    blocks = []
+    for n, (w, b) in enumerate(convs):
+        if n == 0:
+            wp = torch.zeros((w.shape[0], _ALEX_IN_CHANNELS), dtype=torch.float32)
+            wp[:, :w[0].numel()] = w.reshape(w.shape[0], -1)
+            w = wp[:, :, None, None]
+        elif n == 1:
+            w = w.permute(0, 2, 3, 1).reshape(w.shape[0], -1)[:, :, None, None]
+        blocks.append([(ops.pack_weight(w.to(dev).contiguous()), b.to(dev), n < 2)])
+    return blocks

@@ -256,12 +256,12 @@ def evaluate_frames(model, frames: Iterable, size=None, sample_posterior: bool =
     same aligned input frames, and their sums ride in the same download.  MS-SSIM needs frames of at least 161 x 161 px
     as the network sees them; smaller ones raise ``ValueError`` when the first of them arrives.
 
-    `lpips`: a ``metrics.LPIPS`` on the model's device (another device raises ``ValueError`` at the call).  Each piece
-    is then also scored by LPIPS (float64 per frame): ``metrics.LPIPS_LAUNCHES`` kernels per group of frames on the same
-    stream, right after the other metric kernels, on the same aligned input frames; its sums ride in the same download.
-    The VGG activations of one group are freed before the next, so device memory stays flat in the clip's length.
-    LPIPS needs frames of at least 16 x 16 px as the network sees them; smaller ones raise ``ValueError`` when the first
-    of them arrives.
+    `lpips`: a ``metrics.LPIPS`` on the model's device (another device raises ``ValueError`` at the call), on VGG16 or
+    AlexNet features (``lpips.net``).  Each piece is then also scored by LPIPS (float64 per frame): ``lpips.launches``
+    kernels per group of frames on the same stream, right after the other metric kernels, on the same aligned input
+    frames; its sums ride in the same download.  The activations of one group are freed before the next, so device
+    memory stays flat in the clip's length.  LPIPS needs frames of at least ``lpips.min_size`` px on each side as the
+    network sees them (16 for VGG16, 31 for AlexNet); smaller ones raise ``ValueError`` when the first of them arrives.
     """
     from . import metrics
     if lpips is not None:
@@ -334,7 +334,7 @@ def _reconstruct(model, enc: StreamEncoder, dec: StreamDecoder, frames: Iterator
         if ms_ssim:
             out.append(metrics._ms_ssim_scores(extra[0], H, W))
         if lpips is not None:
-            out.append(metrics._lpips_scores(extra[-1], H, W))
+            out.append(metrics._lpips_scores(extra[-1], H, W, lpips.net))
         return tuple(out)
 
     def decode_chunks(latent_chunks) -> None:
@@ -353,7 +353,7 @@ def _reconstruct(model, enc: StreamEncoder, dec: StreamDecoder, frames: Iterator
             if ms_ssim:
                 metrics._check_ms_ssim_size(*seen, "evaluate_frames")
             if lpips is not None:
-                metrics._check_lpips_size(*seen, "evaluate_frames")
+                metrics._check_lpips_size(*seen, "evaluate_frames", lpips.net)
         dev_u8 = io.upload(item)
         if score:
             x, ref = frames_to_input_and_u8(dev_u8, dtype=model.dtype, size=size)

@@ -268,7 +268,7 @@ int64_t cvvae_ms_ssim_workspace_bytes(int32_t T, int32_t H, int32_t W);
  *     weights packed [1][64][32] in the same channel order.  T >= 0 (T == 0 launches nothing), H, W >= 1.  One launch.
  *   the thirteen 3 x 3 convolutions of vgg16.features[0:30] (lpips.py:99-138) through cvvae_conv3d with CVVAE_CONV_RELU, plus
  *     CVVAE_CONV_TF32_OUT on the eight whose output only feeds the next convolution (all but the taps).
- *   cvvae_lpips_tap on each of the five taps relu1_2 .. relu5_3: f fp32 [2T,H,W,C] (C = 64, 128, 256 or 512),
+ *   cvvae_lpips_tap on each of the five taps relu1_2 .. relu5_3: f fp32 [2T,H,W,C] (C = 64, 128, 192, 256, 384 or 512),
  *     lin_w fp32 [C] (the 1x1 head lin{k}, no bias), acc int64 [T] overwritten with, per frame t,
  *       acc[t] = 2^32 * sum over the positions of sum_c w[c] (fa_c / n_a - fb_c / n_b)^2,
  *       n = sqrt(sum_c f_c^2 + 1e-10) + 1e-10   (normalize_tensor, lpips.py:141-143),
@@ -286,6 +286,36 @@ int64_t cvvae_ms_ssim_workspace_bytes(int32_t T, int32_t H, int32_t W);
 int cvvae_lpips_input(const uint8_t* a_thwc, const uint8_t* b_thwc, int32_t T, int32_t H, int32_t W, float* out, void* stream);
 int cvvae_lpips_tap(const float* f, int32_t T, int32_t H, int32_t W, int32_t C, const float* lin_w, int64_t* acc,
                     float* pooled, void* stream);
+/* LPIPS on AlexNet features (lpips v0.1 net='alex', the lpips package's default; torchvision alexnet().features[0:12]):
+ * the same scaling, normalisation, heads and fixed-point sums as above, on five taps relu1 .. relu5 of C = 64, 192, 384,
+ * 256, 256.  The caller runs, for T frame pairs of H x W px (H, W >= 31 for relu5 to have a position):
+ *   cvvae_lpips_alex_input: conv1's input (11 x 11, stride 4, zero padding 2) with its 363 taps packed into channels:
+ *     out fp32 [2T,h1,w1,384], h1 = (H-7)/4 + 1, w1 = (W-7)/4 + 1, 16-byte aligned, images as cvvae_lpips_input.  Channel
+ *     (c*11 + kh)*11 + kw of position (oh, ow) is s(4 oh + kh - 2, 4 ow + kw - 2, c) with s exactly as cvvae_lpips_input
+ *     computes it (TF32-rounded), 0 outside the frame and in channels 363..383: the order of the weight [64,3,11,11]
+ *     flattened, so conv1 runs as a 1 x 1 convolution over 384 channels.  T >= 0 (T == 0 launches nothing), H, W >= 7.
+ *     One launch.
+ *   conv1 (cvvae_conv3d, CVVAE_CONV_RELU) -> relu1 [2T,h1,w1,64], fp32; cvvae_lpips_tap on it without a pool.
+ *   cvvae_lpips_max_pool3s2: the 3 x 3 stride-2 max pool (floor, no padding) of features[2] and [5]: f fp32 [N,H,W,C] ->
+ *     out fp32 [N,(H-3)/2+1,(W-3)/2+1,C], stored rounded to the nearest TF32 value (its only consumer is a convolution).
+ *     N >= 0, H, W >= 3, C % 4 == 0, H*W*C < 2^31, both 16-byte aligned.  One launch.
+ *   cvvae_lpips_pack5x5: conv2's 5 x 5 taps (zero padding 2) packed into channels: x fp32 [N,H,W,C] -> out fp32
+ *     [N,H,W,25C], channel (kh*5 + kw)*C + c of (h, w) is x(h+kh-2, w+kw-2, c), 0 outside the image, an exact copy; conv2
+ *     then runs as a 1 x 1 convolution over 25 * 64 = 1600 channels with its weights packed in that order.  N >= 0,
+ *     H, W >= 1, C % 4 == 0, 25*H*W*C < 2^31, both 16-byte aligned.  One launch.
+ *   conv2 -> relu2 [.., 192] and its tap; the pool; conv3 (3 x 3) -> relu3 [.., 384]; conv4 -> relu4 [.., 256];
+ *     conv5 -> relu5 [.., 256].
+ *   cvvae_lpips_tap_copy on relu3 and relu4: cvvae_lpips_tap (C = 256 or 384, no pool) that also writes `copy` fp32
+ *     [2T,H,W,C], every value of f rounded to the nearest TF32, from the same pass: the input of the next convolution,
+ *     while the tap itself stays fp32.  `copy` must not be NULL.  One launch (plus a memset of acc).
+ *   cvvae_lpips_tap on relu5.  One group of frames costs 14 kernel launches.
+ * Every index in these kernels is 64-bit across images and 32-bit within one (checked above). */
+int cvvae_lpips_alex_input(const uint8_t* a_thwc, const uint8_t* b_thwc, int32_t T, int32_t H, int32_t W, float* out,
+                           void* stream);
+int cvvae_lpips_max_pool3s2(const float* f, int32_t N, int32_t H, int32_t W, int32_t C, float* out, void* stream);
+int cvvae_lpips_pack5x5(const float* x, int32_t N, int32_t H, int32_t W, int32_t C, float* out, void* stream);
+int cvvae_lpips_tap_copy(const float* f, int32_t T, int32_t H, int32_t W, int32_t C, const float* lin_w, int64_t* acc,
+                         float* copy, void* stream);
 
 /* Diagnostics */
 /* Per-CTA phase timestamps of the next conv_tc launches: device buffer of n_ctas x 8 uint64 (globaltimer ns:

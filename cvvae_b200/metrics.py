@@ -44,7 +44,7 @@ symmetric in a and b.  Frames need at least 16 x 16 px (relu5_3 is H/16 x W/16) 
 fixed-point sums).  No weights ship with the package:
 ``LPIPS.from_state_dict`` takes torchvision's VGG16 state dict (or the reference module's) and the lpips heads.
 
-``LPIPS.from_state_dict(..., net="alex")`` is the same metric on AlexNet features, the lpips package's default network
+``LPIPS.from_state_dict(..., net='alex')`` is the same metric on AlexNet features, the lpips package's default network
 (``lpips.LPIPS()``, and the LPIPS column of most published reconstruction tables; the two networks give different
 numbers).  Only the trunk differs: torchvision's ``alexnet().features[0:12]``, i.e. conv1 (11 x 11, stride 4, padding 2)
 -> relu1, a 3 x 3 stride-2 max pool (floor), conv2 (5 x 5, padding 2) -> relu2, the same pool, conv3 .. conv5 (3 x 3,
@@ -55,7 +55,8 @@ frames need at least 31 x 31 px.  The ``spatial=True`` variant (maps upsampled t
 """
 from __future__ import annotations
 
-from typing import NamedTuple
+from types import SimpleNamespace
+from typing import NamedTuple, Optional
 
 import torch
 
@@ -66,22 +67,12 @@ MS_SSIM_WEIGHTS = (0.0448, 0.2856, 0.3001, 0.2363, 0.1333)
 MS_SSIM_MIN_SIZE = 161
 MS_SSIM_LAUNCHES = 9          # per call: five levels scored, four pooling steps
 LPIPS_MIN_SIZE = 16
-LPIPS_LAUNCHES = 19           # per group of frames: the input kernel, 13 convolutions, 5 taps
+LPIPS_ALEX_MIN_SIZE = 31      # AlexNet: relu3 .. relu5 have (p1 - 3) // 2 + 1 >= 1 rows, p1 = ((H - 7) // 4 - 2) // 2 + 1
 LPIPS_MAX_POSITIONS = 1 << 23   # H * W: the range of the tap kernel's fixed-point sums (include/cvvae_b200.h)
-LPIPS_GROUP_BYTES = 8 << 30   # device bytes of VGG activations one group may take: one frame pair at the largest size
+LPIPS_GROUP_BYTES = 8 << 30   # device bytes of activations one group may take: one frame pair at the largest size
 LPIPS_SHIFT = (-0.030, -0.088, -0.188)
 LPIPS_SCALE = (0.458, 0.448, 0.450)
 LPIPS_MAX_HEAD = 32.0         # |w| bound of the heads that keeps the tap kernel's fixed-point sums in range
-# vgg16.features indices of the thirteen convolutions, per block (the reference's slice1 .. slice5); each block ends in a tap
-_VGG_BLOCKS = ((0, 2), (5, 7), (10, 12, 14), (17, 19, 21), (24, 26, 28))
-_VGG_CHANNELS = (64, 128, 256, 512, 512)
-LPIPS_NETS = ("vgg", "alex")
-LPIPS_ALEX_MIN_SIZE = 31      # AlexNet: relu3 .. relu5 have (p1 - 3) // 2 + 1 >= 1 rows, p1 = ((H - 7) // 4 - 2) // 2 + 1
-LPIPS_ALEX_LAUNCHES = 14      # per group of frames: the input kernel, 5 convolutions, 5 taps, 2 pools, conv2's packing
-# alexnet.features index, Cin, kernel extent of the five convolutions (lpips' slice1 .. slice5 hold one each), and the taps
-_ALEX_CONVS = ((0, 3, 11), (3, 64, 5), (6, 192, 3), (8, 384, 3), (10, 256, 3))
-_ALEX_CHANNELS = (64, 192, 384, 256, 256)
-_ALEX_IN_CHANNELS = 384       # conv1's 3 x 11 x 11 = 363 taps, padded to a multiple of the channel block
 
 
 class FrameMetrics(NamedTuple):
@@ -117,15 +108,33 @@ def _check_frames(a: torch.Tensor, b: torch.Tensor, who: str) -> None:
         raise ValueError(f"{who}: `a` and `b` differ: {tuple(a.shape)} on {a.device} vs {tuple(b.shape)} on {b.device}")
 
 
+# A scorer is a metric as evaluate_frames runs it on every piece, and _sums for the per-frame functions (LPIPS is one):
+#   _check(H, W, who)     refuses a frame size before any device work (ValueError naming `who`)
+#   _launch(a, b)         the kernels on the frames' device and current stream: the int64 sums, on the device
+#   _finish(sums, H, W)   those sums on the host -> the float64 [T] tensors a piece of evaluate_frames carries
+#   _empty                the host sums of no frames
+
+
+def _sums(metric, a: torch.Tensor, b: torch.Tensor, who: str) -> torch.Tensor:
+    """`metric`'s size refusal, then its sums of the checked frames `a` and `b`, on the host (no frames: no device work)."""
+    T, H, W, _ = a.shape
+    metric._check(H, W, who)
+    return metric._launch(a.contiguous(), b.contiguous()).cpu() if T else metric._empty
+
+
 def frame_metrics(a: torch.Tensor, b: torch.Tensor) -> FrameMetrics:
     """PSNR, SSIM and squared error of every frame of `b` against the same frame of `a` (both CUDA uint8 [T, H, W, 3])."""
     _check_frames(a, b, "frame_metrics")
-    T, H, W, _ = a.shape
+    _, H, W, _ = a.shape
     if H < _WINDOW or W < _WINDOW:
         raise ValueError(f"frame_metrics: SSIM needs frames of at least {_WINDOW} x {_WINDOW} px; got {H} x {W}")
-    if T == 0:
-        return _scores(torch.empty((0, 2), dtype=torch.int64), H, W)
-    return _scores(_launch(a.contiguous(), b.contiguous()).cpu(), H, W)
+    return _scores(_sums(_PSNR_SSIM, a, b, "frame_metrics"), H, W)
+
+
+# evaluate_frames refuses no size for PSNR / SSIM on arrival: frame_metrics checks the 11 px itself, and in the stream
+# the kernel's entry point refuses smaller frames at the launch
+_PSNR_SSIM = SimpleNamespace(_check=lambda H, W, who: None, _launch=_launch,
+                             _finish=lambda sums, H, W: _scores(sums, H, W)[:2], _empty=torch.empty((0, 2), dtype=torch.int64))
 
 
 def _check_ms_ssim_size(H: int, W: int, who: str) -> None:
@@ -168,32 +177,21 @@ def _ms_ssim_scores(acc: torch.Tensor, H: int, W: int) -> torch.Tensor:
     return factors.pow(w[:, None]).prod(dim=1).mean(dim=1)
 
 
+_MS_SSIM = SimpleNamespace(_check=_check_ms_ssim_size, _launch=_launch_ms_ssim,
+                           _finish=lambda sums, H, W: (_ms_ssim_scores(sums, H, W),),
+                           _empty=torch.empty((0, len(MS_SSIM_WEIGHTS), 3, 2), dtype=torch.int64))
+
+
 def frame_ms_ssim(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
     """Multi-scale SSIM of every frame of `b` against the same frame of `a` (both CUDA uint8 [T, H, W, 3], H, W >= 161):
     float64 [T] on the host.  The module docstring has the definition."""
     _check_frames(a, b, "frame_ms_ssim")
-    T, H, W, _ = a.shape
-    _check_ms_ssim_size(H, W, "frame_ms_ssim")
-    if T == 0:
-        return torch.empty(0, dtype=torch.float64)
-    return _ms_ssim_scores(_launch_ms_ssim(a.contiguous(), b.contiguous()).cpu(), H, W)
-
-
-def _check_lpips_size(H: int, W: int, who: str, net: str = "vgg") -> None:
-    if net == "alex" and min(H, W) < LPIPS_ALEX_MIN_SIZE:
-        raise ValueError(f"{who}: LPIPS (AlexNet) needs frames of at least {LPIPS_ALEX_MIN_SIZE} x {LPIPS_ALEX_MIN_SIZE} px "
-                         f"(its last taps, relu3 .. relu5, follow the stride-4 conv1 and two 3 x 3 stride-2 pools); got "
-                         f"{H} x {W}")
-    if min(H, W) < LPIPS_MIN_SIZE:
-        raise ValueError(f"{who}: LPIPS needs frames of at least {LPIPS_MIN_SIZE} x {LPIPS_MIN_SIZE} px (its last tap, "
-                         f"relu5_3, is 1/16 of the size); got {H} x {W}")
-    if H * W > LPIPS_MAX_POSITIONS:
-        raise ValueError(f"{who}: LPIPS takes frames of at most 2^23 px (the range of its fixed-point sums); got {H} x {W}")
+    return _ms_ssim_scores(_sums(_MS_SSIM, a, b, "frame_ms_ssim"), a.shape[1], a.shape[2])
 
 
 def _lpips_tap_sizes(H: int, W: int) -> list:
-    """(h, w) of the five taps: each block after the first starts with a 2 x 2 max pool, floor."""
-    return [(H >> k, W >> k) for k in range(len(_VGG_BLOCKS))]
+    """(h, w) of VGG16's five taps: each block after the first starts with a 2 x 2 max pool, floor."""
+    return [(H >> k, W >> k) for k in range(5)]
 
 
 def _lpips_alex_tap_sizes(H: int, W: int) -> list:
@@ -207,10 +205,103 @@ def _lpips_alex_tap_sizes(H: int, W: int) -> list:
     return [(h1, w1), (hp1, wp1)] + [(hp2, wp2)] * 3
 
 
+class _Conv(NamedTuple):
+    """One convolution (then ReLU) of an LPIPS trunk.  `pack` None: 'same' 3 x 3; ``(order, Cp)``: 1 x 1 over its taps,
+    which the step before packs into Cp channels, zero-padded, in (kh, kw, c) ("hwc") or (c, kh, kw) ("chw") order."""
+    slice: int           # lpips' net.slice{slice + 1} holds it
+    index: int           # its torchvision ``features`` index
+    cin: int
+    cout: int
+    extent: int          # kernel extent
+    pack: Optional[tuple] = None
+
+
+class _LpipsNet(NamedTuple):
+    """Everything that differs between the LPIPS networks.  `plan`: one kernel launch per step, each reading what the
+    one before left: ("input", fn) packs the scaled frames for conv 0; ("conv", n, tf32_out) is conv n, its output
+    rounded to TF32 if only a convolution reads it; ("tap", k, side) is tap k, also writing the 2 x 2 max pool ("pool2")
+    or a TF32 copy ("copy") for the next convolution; ("max_pool3s2",); ("pack5x5",) packs 5 x 5 taps, (kh, kw, c)."""
+    convs: tuple         # _Conv, in order
+    channels: tuple      # C_k of the taps; their number sizes the accumulator
+    tap_sizes: object    # (H, W) -> [(h, w)] of the taps
+    min_size: int
+    too_small: str       # the refusal of frames under min_size, formatted with who, n = min_size, H and W
+    plan: tuple
+
+    def shapes(self, H: int, W: int) -> list:
+        """(h, w, C) of the activation each step of the plan leaves for the next, for H x W frames."""
+        out, h, w, c = [], H, W, 3
+        for op, *arg in self.plan:
+            if op == "input":
+                (h, w), c = self.tap_sizes(H, W)[0], self.convs[0].pack[1]
+            elif op == "conv":
+                c = self.convs[arg[0]].cout
+            elif op == "tap" and arg[1] == "pool2":
+                h, w = h // 2, w // 2
+            elif op == "max_pool3s2":
+                h, w = (h - 3) // 2 + 1, (w - 3) // 2 + 1
+            elif op == "pack5x5":
+                c *= 25
+            out.append((h, w, c))
+        return out
+
+    def pair_bytes(self, H: int, W: int) -> int:
+        """Device bytes of the largest activations live at once for a frame pair: a convolution's fp32 input and output."""
+        shapes = self.shapes(H, W)
+        return 2 * 4 * max((shapes[n - 1][2] + c) * h * w
+                           for n, ((op, *_), (h, w, c)) in enumerate(zip(self.plan, shapes)) if op == "conv")
+
+
+def _vgg16() -> _LpipsNet:
+    """VGG16 ``features[0:30]``: lpips' five slices of 3 x 3 convolutions, each ending in a tap, 2 x 2 max pools between
+    them.  conv1_1 runs as a 1 x 1 convolution over the 27 taps cvvae_lpips_input packs into 32 channels."""
+    blocks = ((0, 2), (5, 7), (10, 12, 14), (17, 19, 21), (24, 26, 28))   # features indices of the convolutions
+    channels = (64, 128, 256, 512, 512)
+    convs, plan, cin = [], [("input", "cvvae_lpips_input")], 3
+    for k, (block, c) in enumerate(zip(blocks, channels)):
+        for j, i in enumerate(block):
+            # a slice's last convolution is its tap, read as data in fp32; the others only feed the next convolution
+            plan.append(("conv", len(convs), j + 1 < len(block)))
+            convs.append(_Conv(k, i, cin, c, 3, None if convs else ("hwc", 32)))
+            cin = c
+        plan.append(("tap", k, "pool2" if k + 1 < len(blocks) else None))
+    return _LpipsNet(tuple(convs), channels, _lpips_tap_sizes, LPIPS_MIN_SIZE,
+                     "{who}: LPIPS needs frames of at least {n} x {n} px (its last tap, relu5_3, is 1/16 of the size); "
+                     "got {H} x {W}", tuple(plan))
+
+
+_VGG16 = _vgg16()
+# AlexNet features[0:12], one convolution (a tap) per lpips slice.  conv1 and conv2 run as 1 x 1 convolutions over their
+# taps packed into channels; relu3 and relu4 reach the next convolution through the tap kernel's TF32 copy.
+_ALEXNET = _LpipsNet(
+    convs=(_Conv(0, 0, 3, 64, 11, ("chw", 384)), _Conv(1, 3, 64, 192, 5, ("hwc", 1600)), _Conv(2, 6, 192, 384, 3),
+           _Conv(3, 8, 384, 256, 3), _Conv(4, 10, 256, 256, 3)),
+    channels=(64, 192, 384, 256, 256),
+    tap_sizes=_lpips_alex_tap_sizes,
+    min_size=LPIPS_ALEX_MIN_SIZE,
+    too_small="{who}: LPIPS (AlexNet) needs frames of at least {n} x {n} px (its last taps, relu3 .. relu5, follow the "
+              "stride-4 conv1 and two 3 x 3 stride-2 pools); got {H} x {W}",
+    plan=(("input", "cvvae_lpips_alex_input"), ("conv", 0, False), ("tap", 0, None), ("max_pool3s2",), ("pack5x5",),
+          ("conv", 1, False), ("tap", 1, None), ("max_pool3s2",), ("conv", 2, False), ("tap", 2, "copy"),
+          ("conv", 3, False), ("tap", 3, "copy"), ("conv", 4, False), ("tap", 4, None)))
+_NETS = {"vgg": _VGG16, "alex": _ALEXNET}
+LPIPS_NETS = tuple(_NETS)
+LPIPS_LAUNCHES = len(_VGG16.plan)          # per group of frames: the input kernel, 13 convolutions, 5 taps
+LPIPS_ALEX_LAUNCHES = len(_ALEXNET.plan)   # the input kernel, 5 convolutions, 5 taps, 2 pools, conv2's packing
+
+
+def _check_lpips_size(H: int, W: int, who: str, net: str = "vgg") -> None:
+    spec = _NETS[net]
+    if min(H, W) < spec.min_size:
+        raise ValueError(spec.too_small.format(who=who, n=spec.min_size, H=H, W=W))
+    if H * W > LPIPS_MAX_POSITIONS:
+        raise ValueError(f"{who}: LPIPS takes frames of at most 2^23 px (the range of its fixed-point sums); got {H} x {W}")
+
+
 def _lpips_scores(acc: torch.Tensor, H: int, W: int, net: str = "vgg") -> torch.Tensor:
     """Host int64 [5, T] of the tap kernels (per tap and frame, the sum over positions times 2^32) -> LPIPS, float64 [T]."""
     d = torch.zeros(acc.shape[1], dtype=torch.float64)
-    for k, (h, w) in enumerate(_lpips_alex_tap_sizes(H, W) if net == "alex" else _lpips_tap_sizes(H, W)):
+    for k, (h, w) in enumerate(_NETS[net].tap_sizes(H, W)):
         d += acc[k].double() / 4294967296.0 / (h * w)
     return d
 
@@ -244,21 +335,12 @@ def _lpips_weights(state_dicts: tuple, net: str = "vgg") -> tuple:
             v = get((key,), (1, 3, 1, 1))
             if not torch.equal(v.flatten(), torch.tensor(want, dtype=torch.float32)):
                 raise ValueError(f"LPIPS.from_state_dict: {key!r} is {v.flatten().tolist()}, expected {list(want)}")
-    # per convolution: lpips slice k (0-based), features index i, Cin, Cout, kernel extent
-    if net == "alex":
-        layers = [(k, i, cin, c, ks) for k, ((i, cin, ks), c) in enumerate(zip(_ALEX_CONVS, _ALEX_CHANNELS))]
-    else:
-        layers, cin = [], 3
-        for k, (block, c) in enumerate(zip(_VGG_BLOCKS, _VGG_CHANNELS)):
-            for i in block:
-                layers.append((k, i, cin, c, 3))
-                cin = c
     convs = []
-    for k, i, cin, c, ks in layers:
-        keys = lambda s: (f"features.{i}.{s}", f"net.slice{k + 1}.{i}.{s}")   # noqa: E731
-        convs.append((get(keys("weight"), (c, cin, ks, ks)), get(keys("bias"), (c,))))
+    for c in _NETS[net].convs:
+        keys = lambda s: (f"features.{c.index}.{s}", f"net.slice{c.slice + 1}.{c.index}.{s}")   # noqa: E731
+        convs.append((get(keys("weight"), (c.cout, c.cin, c.extent, c.extent)), get(keys("bias"), (c.cout,))))
     heads = []
-    for k, c in enumerate(_ALEX_CHANNELS if net == "alex" else _VGG_CHANNELS):
+    for k, c in enumerate(_NETS[net].channels):
         key = f"lin{k}.model.1.weight"
         v = get((key,), (1, c, 1, 1))
         if v.abs().max().item() > LPIPS_MAX_HEAD:
@@ -269,22 +351,34 @@ def _lpips_weights(state_dicts: tuple, net: str = "vgg") -> tuple:
     return convs, heads
 
 
+def _conv_tc_weight(w: torch.Tensor, pack: Optional[tuple]) -> torch.Tensor:
+    """A weight as conv_tc runs it (see _Conv): unchanged, or [Cout, Cp, 1, 1], the taps in the packing order, zeros after."""
+    if pack is None:
+        return w
+    order, cp = pack
+    taps = (w.permute(0, 2, 3, 1) if order == "hwc" else w).reshape(w.shape[0], -1)
+    out = torch.zeros((w.shape[0], cp), dtype=torch.float32)
+    out[:, :taps.shape[1]] = taps
+    return out[:, :, None, None]
+
+
 class LPIPS:
     """LPIPS (lpips v0.1, VGG16 or AlexNet features) of every frame of `b` against the same frame of `a` on the GPU; the
     module docstring has the definition.  Build it with ``LPIPS.from_state_dict``; ``metric(a, b)`` takes two CUDA uint8
     ``[T, H, W, 3]`` videos on ``metric.device`` (H, W >= ``metric.min_size``, H * W <= 2^23) and returns float64 ``[T]``
-    on the host.  ``metric.net`` is ``"vgg"`` or ``"alex"``.
+    on the host.  ``metric.net`` is ``'vgg'`` or ``'alex'``.
 
     Frames are scored in groups whose activations stay within ``LPIPS_GROUP_BYTES``; each group is ``metric.launches``
     kernel launches on the current stream of the device.  The result is the same, bit for bit, whatever the grouping."""
 
     net = "vgg"   # the network of an instance built without naming one
 
-    def __init__(self, blocks: list, heads: list, device: torch.device, net: str = "vgg"):
+    def __init__(self, convs: list, heads: list, device: torch.device, net: str = "vgg"):   # as _lpips_weights returns them
         from .ops import CudaOps
         self._ops = CudaOps()
-        self._blocks = blocks          # per block: [(packed weight, bias, 1 x 1 tap-packed?)]
-        self._heads = heads            # fp32 [C_k] per tap
+        self._convs = [(self._ops.pack_weight(_conv_tc_weight(w, c.pack).to(device).contiguous()), b.to(device))
+                       for (w, b), c in zip(convs, _NETS[net].convs)]   # the weights as conv_tc reads them
+        self._heads = [h.to(device) for h in heads]                      # fp32 [C_k] per tap
         self.device = device
         self.net = net
         self._group_bytes = LPIPS_GROUP_BYTES
@@ -292,19 +386,19 @@ class LPIPS:
     @property
     def min_size(self) -> int:
         """The smallest frame side the network accepts: 16 px for VGG16, 31 px for AlexNet."""
-        return LPIPS_ALEX_MIN_SIZE if self.net == "alex" else LPIPS_MIN_SIZE
+        return _NETS[self.net].min_size
 
     @property
     def launches(self) -> int:
         """Kernel launches per group of frames."""
-        return LPIPS_ALEX_LAUNCHES if self.net == "alex" else LPIPS_LAUNCHES
+        return len(_NETS[self.net].plan)
 
     @classmethod
     def from_state_dict(cls, *state_dicts, device=None, net: str = "vgg") -> "LPIPS":
         """Weights from one or more state dicts, merged (later ones win).  ``net="vgg"`` (the default): the thirteen
         convolutions under torchvision's keys ``features.{i}.weight`` / ``.bias`` (``vgg16-397923af.pth``) or the
         reference module's ``net.slice{k}.{i}.*`` (same i), the heads under ``lin{k}.model.1.weight`` ``[1, C_k, 1, 1]``
-        (lpips v0.1 ``vgg.pth``, or the reference's ``LPIPS().state_dict()``).  ``net="alex"``, the lpips package's
+        (lpips v0.1 ``vgg.pth``, or the reference's ``LPIPS().state_dict()``).  ``net='alex'``, the lpips package's
         default network: the five convolutions ``features.{0,3,6,8,10}.*`` of torchvision's AlexNet
         (``alexnet-owt-7be5be79.pth``) or the lpips module's ``net.slice{k}.{i}.*``, and the heads of lpips v0.1
         ``alex.pth`` (C_k = 64, 192, 384, 256, 256).  ``scaling_layer.shift`` / ``.scale``, if present, must be the
@@ -319,144 +413,62 @@ class LPIPS:
             raise ValueError(f"LPIPS.from_state_dict: the device must be a CUDA device, got {dev}")
         if dev is None or dev.index is None:
             dev = torch.device("cuda", torch.cuda.current_device() if dev is None or dev.index is None else dev.index)
-        from .ops import CudaOps
-        ops = CudaOps()
-        if net == "alex":
-            return cls(_alex_blocks(ops, convs, dev), [h.to(dev) for h in heads], dev, net)
-        blocks, n = [], 0
-        for k, block in enumerate(_VGG_BLOCKS):
-            layers = []
-            for _ in block:
-                w, b = convs[n]
-                if n == 0:   # conv1_1 as a 1 x 1 convolution over the 32 tap-packed channels of cvvae_lpips_input
-                    wp = torch.zeros((w.shape[0], 32), dtype=torch.float32)
-                    wp[:, :27] = w.permute(0, 2, 3, 1).reshape(w.shape[0], 27)
-                    w = wp[:, :, None, None]
-                layers.append((ops.pack_weight(w.to(dev).contiguous()), b.to(dev), n == 0))
-                n += 1
-            blocks.append(layers)
-        m = cls(blocks, [h.to(dev) for h in heads], dev)
-        return m
+        return cls(convs, heads, dev, net)
 
     def _group(self, H: int, W: int) -> int:
-        """Frames per group.  VGG16: the largest activations live at once are conv1_2's input and output, 64 + 64 fp32
-        channels at full size for both videos.  AlexNet: conv1's packed input and output (384 + 64 channels) or conv2's
-        (1600 + 192), whichever is larger."""
-        if self.net == "alex":
-            (h1, w1), (h2, w2) = _lpips_alex_tap_sizes(H, W)[:2]
-            return max(1, self._group_bytes // (2 * 4 * max((_ALEX_IN_CHANNELS + 64) * h1 * w1, (1600 + 192) * h2 * w2)))
-        return max(1, self._group_bytes // (2 * 128 * 4 * H * W))
+        """Frames per group: the budget over a frame pair's largest live activations (VGG16: conv1_2's input and output;
+        AlexNet: conv1's or conv2's)."""
+        return max(1, self._group_bytes // _NETS[self.net].pair_bytes(H, W))
+
+    def _check(self, H: int, W: int, who: str) -> None:
+        _check_lpips_size(H, W, who, self.net)
 
     @L._on_tensor_device
     def _launch(self, a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
         """The kernels on the current stream of the frames' device: int64 [5, T] (per tap and frame, the sum over
         positions of the weighted squared difference times 2^32), on the device."""
         T, H, W, _ = a.shape
-        acc = torch.empty((len(_VGG_BLOCKS), T), dtype=torch.int64, device=a.device)
+        acc = torch.empty((len(_NETS[self.net].channels), T), dtype=torch.int64, device=a.device)
         g = self._group(H, W)
         for t0 in range(0, T, g):
             self._run_group(a[t0:t0 + g], b[t0:t0 + g], acc[:, t0:t0 + g])
         return acc
 
+    def _finish(self, sums: torch.Tensor, H: int, W: int) -> tuple:
+        return (_lpips_scores(sums, H, W, self.net),)
+
+    @property
+    def _empty(self) -> torch.Tensor:
+        return torch.empty((len(_NETS[self.net].channels), 0), dtype=torch.int64)
+
     def _run_group(self, a: torch.Tensor, b: torch.Tensor, acc: torch.Tensor) -> None:
-        if self.net == "alex":
-            return self._run_group_alex(a, b, acc)
+        """The network's plan on one group of frame pairs, both videos as one batch of 2G images.  Only the activation
+        the next step reads stays alive: each step's output replaces it, a tap without a side output leaves it."""
         G, H, W, _ = a.shape
-        lib, dev, stream = self._ops.lib, a.device, L._stream(a)
-        x = torch.empty((2 * G, 1, H, W, 32), dtype=torch.float32, device=dev)
-        L.check(lib.cvvae_lpips_input(a.data_ptr(), b.data_ptr(), G, H, W, x.data_ptr(), stream), "cvvae_lpips_input")
-        h, w = H, W
-        for k, layers in enumerate(self._blocks):
-            for j, (wp, bias, packed_taps) in enumerate(layers):
-                y = torch.empty((2 * G, 1, h, w, wp.shape[1]), dtype=torch.float32, device=dev)
-                # a block's last convolution is a tap, read as data in fp32; the others only feed the next convolution
-                # and are stored rounded to TF32, as the tensor cores should read them
-                kw = dict(relu=True, tf32_out=j + 1 < len(layers))
-                if packed_taps:
-                    self._ops.conv(x, wp, bias, out=y, **kw)
-                else:
-                    self._ops.conv(x, wp, bias, kernel=(1, 3, 3), offset=(0, -1, -1), out=y, **kw)
+        net, lib, stream = _NETS[self.net], self._ops.lib, L._stream(a)
+        x = None
+        for (op, *arg), shape in zip(net.plan, net.shapes(H, W)):
+            y = (None if op == "tap" and arg[1] is None else
+                 torch.empty((2 * G, 1, *shape), dtype=torch.float32, device=a.device))
+            if op == "input":
+                L.check(getattr(lib, arg[0])(a.data_ptr(), b.data_ptr(), G, H, W, y.data_ptr(), stream), arg[0])
+            elif op == "conv":
+                (wp, bias), same3x3 = self._convs[arg[0]], net.convs[arg[0]].pack is None
+                kw = dict(kernel=(1, 3, 3), offset=(0, -1, -1)) if same3x3 else {}
+                self._ops.conv(x, wp, bias, out=y, relu=True, tf32_out=arg[1], **kw)
+            elif op == "tap":
+                k, side = arg
+                fn = "cvvae_lpips_tap_copy" if side == "copy" else "cvvae_lpips_tap"
+                L.check(getattr(lib, fn)(x.data_ptr(), G, *x.shape[2:], self._heads[k].data_ptr(), acc[k].data_ptr(),
+                                         None if y is None else y.data_ptr(), stream), fn)
+            else:   # max_pool3s2, pack5x5: image by image
+                fn = "cvvae_lpips_" + op
+                L.check(getattr(lib, fn)(x.data_ptr(), 2 * G, *x.shape[2:], y.data_ptr(), stream), fn)
+            if y is not None:
                 x = y
-            C = x.shape[-1]
-            pooled = (torch.empty((2 * G, 1, h // 2, w // 2, C), dtype=torch.float32, device=dev)
-                      if k + 1 < len(self._blocks) else None)
-            L.check(lib.cvvae_lpips_tap(x.data_ptr(), G, h, w, C, self._heads[k].data_ptr(), acc[k].data_ptr(),
-                                        None if pooled is None else pooled.data_ptr(), stream), "cvvae_lpips_tap")
-            if pooled is not None:
-                x, h, w = pooled, h // 2, w // 2
-
-    def _run_group_alex(self, a: torch.Tensor, b: torch.Tensor, acc: torch.Tensor) -> None:
-        """AlexNet's features[0:12] on both videos, every convolution output a tap (fp32); what only a convolution reads
-        is TF32: conv1's packed input, the pools (hence conv2's packed input) and the copies of relu3 and relu4."""
-        G, H, W, _ = a.shape
-        lib, dev, stream = self._ops.lib, a.device, L._stream(a)
-        sizes = _lpips_alex_tap_sizes(H, W)
-        convs = [block[0][:2] for block in self._blocks]   # (packed weight, bias) of conv1 .. conv5
-
-        def conv(x, wp, bias, k, three_by_three):
-            y = torch.empty((2 * G, 1, *sizes[k], wp.shape[1]), dtype=torch.float32, device=dev)
-            if three_by_three:
-                return self._ops.conv(x, wp, bias, kernel=(1, 3, 3), offset=(0, -1, -1), out=y, relu=True)
-            return self._ops.conv(x, wp, bias, out=y, relu=True)
-
-        def tap(f, k, copy=None):
-            h, w = sizes[k]
-            args = (f.data_ptr(), G, h, w, f.shape[-1], self._heads[k].data_ptr(), acc[k].data_ptr())
-            if copy is None:
-                L.check(lib.cvvae_lpips_tap(*args, None, stream), "cvvae_lpips_tap")
-            else:
-                L.check(lib.cvvae_lpips_tap_copy(*args, copy.data_ptr(), stream), "cvvae_lpips_tap_copy")
-
-        def pool(f, k):
-            (h, w), (oh, ow) = sizes[k], sizes[k + 1]
-            out = torch.empty((2 * G, 1, oh, ow, f.shape[-1]), dtype=torch.float32, device=dev)
-            L.check(lib.cvvae_lpips_max_pool3s2(f.data_ptr(), 2 * G, h, w, f.shape[-1], out.data_ptr(), stream),
-                    "cvvae_lpips_max_pool3s2")
-            return out
-
-        x = torch.empty((2 * G, 1, *sizes[0], _ALEX_IN_CHANNELS), dtype=torch.float32, device=dev)
-        L.check(lib.cvvae_lpips_alex_input(a.data_ptr(), b.data_ptr(), G, H, W, x.data_ptr(), stream),
-                "cvvae_lpips_alex_input")
-        f = conv(x, *convs[0], 0, False)
-        del x
-        tap(f, 0)
-        p = pool(f, 0)
-        del f
-        x = torch.empty((2 * G, 1, *sizes[1], 25 * p.shape[-1]), dtype=torch.float32, device=dev)
-        L.check(lib.cvvae_lpips_pack5x5(p.data_ptr(), 2 * G, *sizes[1], p.shape[-1], x.data_ptr(), stream),
-                "cvvae_lpips_pack5x5")
-        del p
-        f = conv(x, *convs[1], 1, False)
-        del x
-        tap(f, 1)
-        x = pool(f, 1)
-        for k in (2, 3, 4):
-            f = conv(x, *convs[k], k, True)
-            x = torch.empty_like(f) if k < 4 else None   # relu3 and relu4 feed the next convolution: their TF32 copy
-            tap(f, k, x)
 
     def __call__(self, a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
         _check_frames(a, b, "LPIPS")
         if a.device != self.device:
             raise ValueError(f"LPIPS: the frames are on {a.device}, the weights on {self.device}")
-        T, H, W, _ = a.shape
-        _check_lpips_size(H, W, "LPIPS", self.net)
-        if T == 0:
-            return torch.empty(0, dtype=torch.float64)
-        return _lpips_scores(self._launch(a.contiguous(), b.contiguous()).cpu(), H, W, self.net)
-
-
-def _alex_blocks(ops, convs: list, dev: torch.device) -> list:
-    """AlexNet's five convolutions packed for conv_tc, one per block ([(packed weight, bias, 1 x 1 tap-packed?)]):
-    conv1 as a 1 x 1 convolution over the 384 channels of cvvae_lpips_alex_input ((c, kh, kw) order, zero-padded),
-    conv2 as one over the 1600 of cvvae_lpips_pack5x5 ((kh, kw, c) order), conv3 .. conv5 as 3 x 3 convolutions."""
-    blocks = []
-    for n, (w, b) in enumerate(convs):
-        if n == 0:
-            wp = torch.zeros((w.shape[0], _ALEX_IN_CHANNELS), dtype=torch.float32)
-            wp[:, :w[0].numel()] = w.reshape(w.shape[0], -1)
-            w = wp[:, :, None, None]
-        elif n == 1:
-            w = w.permute(0, 2, 3, 1).reshape(w.shape[0], -1)[:, :, None, None]
-        blocks.append([(ops.pack_weight(w.to(dev).contiguous()), b.to(dev), n < 2)])
-    return blocks
+        return _lpips_scores(_sums(self, a, b, "LPIPS"), a.shape[1], a.shape[2], self.net)

@@ -231,7 +231,7 @@ def reconstruct_frames(model, frames: Iterable, size=None, sample_posterior: boo
     and bfloat16 models are supported (the pixel conversion kernels are 16-bit).
     """
     enc, dec = _open(model, "reconstruct_frames")
-    return _reconstruct(model, enc, dec, iter(frames), size, sample_posterior, generator, False, False, None)
+    return _reconstruct(model, enc, dec, iter(frames), size, sample_posterior, generator, [])
 
 
 def evaluate_frames(model, frames: Iterable, size=None, sample_posterior: bool = False,
@@ -270,7 +270,8 @@ def evaluate_frames(model, frames: Iterable, size=None, sample_posterior: bool =
         if lpips.device != model.device:
             raise ValueError(f"evaluate_frames: the LPIPS weights are on {lpips.device}, the model on {model.device}")
     enc, dec = _open(model, "evaluate_frames")
-    return _reconstruct(model, enc, dec, iter(frames), size, sample_posterior, generator, True, bool(ms_ssim), lpips)
+    scorers = [metrics._PSNR_SSIM] + ([metrics._MS_SSIM] if ms_ssim else []) + ([lpips] if lpips is not None else [])
+    return _reconstruct(model, enc, dec, iter(frames), size, sample_posterior, generator, scorers)
 
 
 def _open(model, who: str):
@@ -282,10 +283,9 @@ def _open(model, who: str):
 
 
 def _reconstruct(model, enc: StreamEncoder, dec: StreamDecoder, frames: Iterator, size, sample_posterior: bool,
-                 generator, score: bool, ms_ssim: bool, lpips) -> Iterator:
-    """The stream behind reconstruct_frames (`score` False: yields frames) and evaluate_frames (True: yields
-    (frames, psnr, ssim), then ms_ssim with `ms_ssim`, then the LPIPS with an `lpips` metric)."""
-    from . import metrics
+                 generator, scorers: list) -> Iterator:
+    """The stream behind reconstruct_frames (no `scorers`: yields frames) and evaluate_frames (yields the frames, then
+    what each of `scorers`, metrics' scorers, finishes for them)."""
     from .video_io import frames_to_input, frames_to_input_and_u8, output_to_frames
 
     # No device context is held across the yields (it would leak into the caller's code): every allocation, stream and
@@ -311,31 +311,20 @@ def _reconstruct(model, enc: StreamEncoder, dec: StreamDecoder, frames: Iterator
 
     def download(x: torch.Tensor) -> None:
         u8 = output_to_frames(x)
-        if not score:
+        if not scorers:
             return io.download(u8)
         ref = take_refs(u8.shape[0])
         if ref.shape != u8.shape:
             raise ValueError(f"evaluate_frames: the networks return {u8.shape[1]} x {u8.shape[2]} frames for an input of "
                              f"{ref.shape[1]} x {ref.shape[2]}, and frames of different sizes cannot be scored; pass "
                              "`size=` with a size the networks reproduce (a multiple of their spatial stride)")
-        sums = [metrics._launch(ref, u8)]
-        if ms_ssim:
-            sums.append(metrics._launch_ms_ssim(ref, u8))
-        if lpips is not None:
-            sums.append(lpips._launch(ref, u8))
-        io.download(u8, *sums)
+        io.download(u8, *[m._launch(ref, u8) for m in scorers])
 
-    def piece(host: torch.Tensor, sums: Optional[torch.Tensor] = None, *extra: torch.Tensor):
-        if sums is None:
+    def piece(host: torch.Tensor, *sums: torch.Tensor):
+        if not scorers:
             return host
         H, W = host.shape[1], host.shape[2]
-        m = metrics._scores(sums, H, W)
-        out = [host, m.psnr, m.ssim]
-        if ms_ssim:
-            out.append(metrics._ms_ssim_scores(extra[0], H, W))
-        if lpips is not None:
-            out.append(metrics._lpips_scores(extra[-1], H, W, lpips.net))
-        return tuple(out)
+        return (host,) + tuple(v for m, s in zip(scorers, sums) for v in m._finish(s, H, W))
 
     def decode_chunks(latent_chunks) -> None:
         for post in latent_chunks:
@@ -344,18 +333,15 @@ def _reconstruct(model, enc: StreamEncoder, dec: StreamDecoder, frames: Iterator
                 download(x)
 
     for item in frames:
-        item = _host_frames(item, "evaluate_frames" if score else "reconstruct_frames", 0)
+        item = _host_frames(item, "evaluate_frames" if scorers else "reconstruct_frames", 0)
         t = item.shape[0]
         if t == 0:
             continue
-        if ms_ssim or lpips is not None:
-            seen = (int(size[0]), int(size[1])) if size is not None else tuple(item.shape[1:3])
-            if ms_ssim:
-                metrics._check_ms_ssim_size(*seen, "evaluate_frames")
-            if lpips is not None:
-                metrics._check_lpips_size(*seen, "evaluate_frames", lpips.net)
+        seen = (int(size[0]), int(size[1])) if size is not None else tuple(item.shape[1:3])   # as the network sees them
+        for m in scorers:
+            m._check(*seen, "evaluate_frames")
         dev_u8 = io.upload(item)
-        if score:
+        if scorers:
             x, ref = frames_to_input_and_u8(dev_u8, dtype=model.dtype, size=size)
             refs.append(ref)
         else:

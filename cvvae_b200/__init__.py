@@ -10,17 +10,18 @@ Datasets of clip latents back to uint8 videos, batched, in float16, bfloat16 or 
     decode_clips, batch_to_frames
 Reconstruction quality on the device (cvvae_b200/metrics.py): per-frame PSNR / SSIM, multi-scale SSIM and LPIPS (VGG16 or,
 with ``net="alex"``, AlexNet; weights from a state dict) of uint8 videos, and the reconstruction stream with every frame scored (MS-SSIM with
-``ms_ssim=True``, LPIPS with ``lpips=LPIPS.from_state_dict(...)``):
-    frame_metrics, FrameMetrics, frame_ms_ssim, LPIPS, evaluate_frames
+``ms_ssim=True``, LPIPS with ``lpips=LPIPS.from_state_dict(...)``), and where frames differ: per-position SSIM maps,
+LPIPS maps (``LPIPS.map``) and ``evaluate_frames(..., maps=True)``:
+    frame_metrics, FrameMetrics, frame_ms_ssim, ssim_map, LPIPS, evaluate_frames
 """
 from .modeling_vae import (AutoencoderKLOutput, CVVAEModel, CVVAESD3Model, DecoderOutput,
                            DiagonalGaussianDistribution)
-from .metrics import LPIPS, FrameMetrics, frame_metrics, frame_ms_ssim
+from .metrics import LPIPS, FrameMetrics, frame_metrics, frame_ms_ssim, ssim_map
 from .streaming import StreamDecoder, StreamEncoder, decode_clips, encode_clips, evaluate_frames, reconstruct_frames
 from .video_io import batch_to_frames, frames_to_training_input
 
 __all__ = ["CVVAEModel", "CVVAESD3Model", "DecoderOutput", "AutoencoderKLOutput", "DiagonalGaussianDistribution",
            "StreamEncoder", "StreamDecoder", "reconstruct_frames", "evaluate_frames",
            "encode_clips", "frames_to_training_input", "decode_clips", "batch_to_frames", "frame_metrics", "FrameMetrics",
-           "frame_ms_ssim", "LPIPS"]
+           "frame_ms_ssim", "ssim_map", "LPIPS"]
 __version__ = "0.1.0"

@@ -81,6 +81,12 @@ _SIGNATURES = {
     "cvvae_lpips_pack5x5": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "cvvae_lpips_tap_copy": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.c_void_p]),
+    "cvvae_frame_ssim_map": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                       C.c_void_p]),
+    "cvvae_lpips_tap_map": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "cvvae_lpips_upsample_sum": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.c_void_p,
+                                           C.c_void_p]),
     "cvvae_conv_tc_set_trace": (C.c_int, [C.c_void_p, C.c_int32]),
     "cvvae_conv_tc_plan": (C.c_int, [C.POINTER(ConvDesc), C.POINTER(C.c_int32), C.c_int32]),
     "cvvae_last_error": (C.c_char_p, []),

@@ -17,6 +17,10 @@
 // (5 x 5) as 1 x 1 convolutions over their taps packed into channels by lpips_alex_input_kernel (from the uint8 frames,
 // 384 channels) and lpips_pack5x5_kernel (1600 channels), with lpips_max_pool3s2_kernel for the 3 x 3 stride-2 pools.
 //
+// LPIPS maps (lpips spatial=True, either network): lpips_tap_map_kernel is the tap pass, with its pool or copy, that also
+// keeps every position's weighted difference in an fp64 tap map; lpips_upsample_sum_kernel then upsamples the five tap
+// maps bilinearly to the frame and sums them.  The frame sums run exactly as without maps, so the scalar is unchanged.
+//
 // The normalisation and the difference are fp64: a good reconstruction's f_a / |f_a| - f_b / |f_b| is small next to
 // either term, and fp32 would leave a relative error of 1e-7 / |difference| in it.  Accumulation: a warp keeps one
 // fp64 partial per lane over its positions, a CTA reduces its warps in a fixed order and adds its sum, rounded once to
@@ -213,9 +217,13 @@ __device__ __forceinline__ double warp_sum(double v) {
 // CTA (t, blk) owns quads [blk * 32, blk * 32 + 32) of frame t in row-major quad order; warp w of it quads 4w .. 4w + 3.
 // kCopy: `pooled` is instead `copy` [2T, H, W, C], which receives every position of f rounded to the nearest TF32 value
 // (a tap whose next consumer is a convolution, AlexNet's relu3 and relu4); there is no pool.
-template <int C, bool kCopy>
+// kMap: also map [T, H, W] (fp64) = each position's weighted squared difference, summed in its own fp64 accumulator (the
+// lane's channels, then the warp) and stored by lane 0; `part`, the frame sum's accumulator, runs exactly as without it.
+// The map is exactly 0 where the features agree and the same bits with a and b swapped.
+template <int C, bool kCopy, bool kMap = false>
 __device__ __forceinline__ void lpips_tap(const float* __restrict__ f, int T, int H, int W, const float* __restrict__ lin_w,
-                                          unsigned long long* __restrict__ acc, float* __restrict__ pooled, int ctas_per_frame) {
+                                          unsigned long long* __restrict__ acc, float* __restrict__ pooled, int ctas_per_frame,
+                                          double* __restrict__ map = nullptr) {
   constexpr int kV = C / 32;
   __shared__ double s_red[kLpTapThreads / 32];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -268,12 +276,24 @@ __device__ __forceinline__ void lpips_tap(const float* __restrict__ f, int T, in
       sb = warp_sum(sb);
       // f / (sqrt(sum f^2 + 1e-10) + 1e-10), lpips.py:141-143, as a product with the reciprocal
       const double ra = 1.0 / (sqrt(sa + 1e-10) + 1e-10), rb = 1.0 / (sqrt(sb + 1e-10) + 1e-10);
+      double pos = 0.0;
 #pragma unroll
       for (int k = 0; k < kV; ++k) {
         const double d = static_cast<double>(va[k]) * ra - static_cast<double>(vb[k]) * rb;
         part = fma(wc[k], d * d, part);
+        if constexpr (kMap) {
+          // d again with explicit roundings: the compiler may fuse d's product and difference into one FMA, which leaves
+          // the rounding error of the other product (about 1e-17) where a and b agree.  The frame sum rounds that away,
+          // a map would show it; this d is exactly 0 for equal features and exactly -d with a and b swapped.
+          const double dm = __dsub_rn(__dmul_rn(static_cast<double>(va[k]), ra), __dmul_rn(static_cast<double>(vb[k]), rb));
+          pos = fma(wc[k], dm * dm, pos);
+        }
         ma[k] = fmaxf(ma[k], va[k]);
         mb[k] = fmaxf(mb[k], vb[k]);
+      }
+      if constexpr (kMap) {
+        pos = warp_sum(pos);
+        if (lane == 0) map[(static_cast<long long>(t) * H + h) * W + w] = pos;
       }
     }
     if (!kCopy && pooled && full) {
@@ -312,6 +332,71 @@ __global__ void __launch_bounds__(kLpTapThreads, C >= 384 ? 1 : 2)
                           unsigned long long* __restrict__ acc, float* __restrict__ copy, int ctas_per_frame) {
   lpips_tap<C, true>(f, T, H, W, lin_w, acc, copy, ctas_per_frame);
 }
+// either of the above (kCopy: `side` is `copy`, else `pooled`) that also writes the tap's map
+template <int C, bool kCopy>
+__global__ void __launch_bounds__(kLpTapThreads, C >= 384 ? 1 : 2)
+    lpips_tap_map_kernel(const float* __restrict__ f, int T, int H, int W, const float* __restrict__ lin_w,
+                         unsigned long long* __restrict__ acc, float* __restrict__ side, int ctas_per_frame,
+                         double* __restrict__ map) {
+  lpips_tap<C, kCopy, true>(f, T, H, W, lin_w, acc, side, ctas_per_frame, map);
+}
+
+// One tap kernel of the family the entry point selects: plain, with the TF32 copy, or (kMap) either one with the map.
+template <int C, bool kCopy, bool kMap>
+void lpips_tap_kernel_launch(unsigned grid, cudaStream_t stream, const float* f, int T, int H, int W, const float* lin_w,
+                             unsigned long long* acc, float* side, int ctas_per_frame, double* map) {
+  if constexpr (kMap)
+    lpips_tap_map_kernel<C, kCopy><<<grid, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, acc, side, ctas_per_frame, map);
+  else if constexpr (kCopy)
+    lpips_tap_copy_kernel<C><<<grid, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, acc, side, ctas_per_frame);
+  else
+    lpips_tap_kernel<C><<<grid, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, acc, side, ctas_per_frame);
+}
+
+// The taps' maps upsampled to the frame and summed, lpips' spatial=True: out [T, H, W] fp32 = sum over k of the bilinear
+// upsampling (align_corners=False) of tap map k, maps [T, h_k, w_k] fp64 back to back in `taps` from offset off[k].
+// Source positions follow PyTorch's rule for fp32 tensors (scale = in / out, src = max(scale (dst + 0.5) - 0.5, 0), each
+// an fp32 rounding; i0 = floor, i1 = i0 + 1 clamped to in - 1, lambda = src - i0); the interpolation and the sum are fp64,
+// rounded to fp32 once.  One thread per output pixel.
+constexpr int kLpMaps = 5;
+constexpr int kLpUpThreads = 256;
+struct LpTapMaps {
+  int h[kLpMaps], w[kLpMaps];
+  long long off[kLpMaps];
+};
+
+__device__ __forceinline__ void lp_source(int dst, int in, int out, int& i0, int& i1, double& lambda) {
+  const float scale = __fdiv_rn(static_cast<float>(in), static_cast<float>(out));
+  const float src = fmaxf(__fsub_rn(__fmul_rn(scale, __fadd_rn(static_cast<float>(dst), 0.5f)), 0.5f), 0.f);
+  i0 = static_cast<int>(src);
+  i1 = i0 + (i0 < in - 1 ? 1 : 0);
+  lambda = static_cast<double>(__fsub_rn(src, static_cast<float>(i0)));
+}
+
+__global__ void __launch_bounds__(kLpUpThreads)
+    lpips_upsample_sum_kernel(const double* __restrict__ taps, int H, int W, long long n, LpTapMaps m, float* __restrict__ out) {
+  const long long i = static_cast<long long>(blockIdx.x) * kLpUpThreads + threadIdx.x;
+  if (i >= n) return;
+  const int x = static_cast<int>(i % W);
+  const long long r = i / W;
+  const int y = static_cast<int>(r % H);
+  const long long t = r / H;
+  double sum = 0.0;
+#pragma unroll
+  for (int k = 0; k < kLpMaps; ++k) {
+    int y0, y1, x0, x1;
+    double ly, lx;
+    lp_source(y, m.h[k], H, y0, y1, ly);
+    lp_source(x, m.w[k], W, x0, x1, lx);
+    const double* p = taps + m.off[k] + t * m.h[k] * m.w[k];
+    const double* p0 = p + static_cast<long long>(y0) * m.w[k];
+    const double* p1 = p + static_cast<long long>(y1) * m.w[k];
+    const double top = (1.0 - lx) * __ldg(p0 + x0) + lx * __ldg(p0 + x1);
+    const double bot = (1.0 - lx) * __ldg(p1 + x0) + lx * __ldg(p1 + x1);
+    sum += (1.0 - ly) * top + ly * bot;
+  }
+  out[i] = static_cast<float>(sum);
+}
 
 // y extent of the pixel kernels' grids: images are walked along y, 32-bit indices within an image along x
 inline dim3 lp_image_grid(int per_image, long long images) {
@@ -319,12 +404,14 @@ inline dim3 lp_image_grid(int per_image, long long images) {
               static_cast<unsigned>(images < 65535 ? images : 65535));
 }
 
-// the checks and launch shared by cvvae_lpips_tap (pooled: NULL or the 2 x 2 pool) and cvvae_lpips_tap_copy
-template <bool kCopy>
+// the checks and launch shared by cvvae_lpips_tap (pooled: NULL or the 2 x 2 pool), cvvae_lpips_tap_copy and, with kMap,
+// cvvae_lpips_tap_map (map required)
+template <bool kCopy, bool kMap = false>
 int lpips_tap_launch(const char* who, const float* f, int32_t T, int32_t H, int32_t W, int32_t C, const float* lin_w,
-                     int64_t* acc, float* pooled, void* stream_) {
+                     int64_t* acc, float* pooled, void* stream_, double* map = nullptr) {
   const char* side = kCopy ? "copy" : "pooled";
-  CVVAE_CHECK_ARG(f && lin_w && acc && (!kCopy || pooled), "%s: null pointer", who);
+  CVVAE_CHECK_ARG(f && lin_w && acc && (!kCopy || pooled) && (!kMap || map), "%s: null pointer", who);
+  if (kMap) CVVAE_CHECK_ARG(reinterpret_cast<uintptr_t>(map) % sizeof(double) == 0, "%s: `map` must be 8-byte aligned", who);
   if (kCopy)
     CVVAE_CHECK_ARG(C == 256 || C == 384, "%s: C must be 256 or 384, got %d", who, (int)C);
   else
@@ -349,15 +436,15 @@ int lpips_tap_launch(const char* who, const float* f, int32_t T, int32_t H, int3
   const unsigned g = static_cast<unsigned>(grid);
   const int pf = static_cast<int>(per_frame);
   if constexpr (kCopy) {
-    if (C == 256) lpips_tap_copy_kernel<256><<<g, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, out, pooled, pf);
-    else lpips_tap_copy_kernel<384><<<g, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, out, pooled, pf);
+    if (C == 256) lpips_tap_kernel_launch<256, true, kMap>(g, stream, f, T, H, W, lin_w, out, pooled, pf, map);
+    else lpips_tap_kernel_launch<384, true, kMap>(g, stream, f, T, H, W, lin_w, out, pooled, pf, map);
   } else {
-    if (C == 64) lpips_tap_kernel<64><<<g, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, out, pooled, pf);
-    else if (C == 128) lpips_tap_kernel<128><<<g, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, out, pooled, pf);
-    else if (C == 192) lpips_tap_kernel<192><<<g, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, out, pooled, pf);
-    else if (C == 256) lpips_tap_kernel<256><<<g, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, out, pooled, pf);
-    else if (C == 384) lpips_tap_kernel<384><<<g, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, out, pooled, pf);
-    else lpips_tap_kernel<512><<<g, kLpTapThreads, 0, stream>>>(f, T, H, W, lin_w, out, pooled, pf);
+    if (C == 64) lpips_tap_kernel_launch<64, false, kMap>(g, stream, f, T, H, W, lin_w, out, pooled, pf, map);
+    else if (C == 128) lpips_tap_kernel_launch<128, false, kMap>(g, stream, f, T, H, W, lin_w, out, pooled, pf, map);
+    else if (C == 192) lpips_tap_kernel_launch<192, false, kMap>(g, stream, f, T, H, W, lin_w, out, pooled, pf, map);
+    else if (C == 256) lpips_tap_kernel_launch<256, false, kMap>(g, stream, f, T, H, W, lin_w, out, pooled, pf, map);
+    else if (C == 384) lpips_tap_kernel_launch<384, false, kMap>(g, stream, f, T, H, W, lin_w, out, pooled, pf, map);
+    else lpips_tap_kernel_launch<512, false, kMap>(g, stream, f, T, H, W, lin_w, out, pooled, pf, map);
   }
   CVVAE_LAUNCH_CHECK();
   return CVVAE_OK;
@@ -391,6 +478,41 @@ extern "C" int cvvae_lpips_tap(const float* f, int32_t T, int32_t H, int32_t W, 
 extern "C" int cvvae_lpips_tap_copy(const float* f, int32_t T, int32_t H, int32_t W, int32_t C, const float* lin_w,
                                     int64_t* acc, float* copy, void* stream) {
   return lpips_tap_launch<true>("cvvae_lpips_tap_copy", f, T, H, W, C, lin_w, acc, copy, stream);
+}
+
+extern "C" int cvvae_lpips_tap_map(const float* f, int32_t T, int32_t H, int32_t W, int32_t C, const float* lin_w,
+                                   int64_t* acc, float* pooled, float* copy, double* map, void* stream) {
+  CVVAE_CHECK_ARG(!(pooled && copy), "cvvae_lpips_tap_map: at most one of pooled and copy may be set");
+  if (copy) return lpips_tap_launch<true, true>("cvvae_lpips_tap_map", f, T, H, W, C, lin_w, acc, copy, stream, map);
+  return lpips_tap_launch<false, true>("cvvae_lpips_tap_map", f, T, H, W, C, lin_w, acc, pooled, stream, map);
+}
+
+extern "C" int cvvae_lpips_upsample_sum(const double* taps, int32_t T, int32_t H, int32_t W, const int32_t* tap_hw, float* out,
+                                        void* stream) {
+  CVVAE_CHECK_ARG(taps && tap_hw && out, "cvvae_lpips_upsample_sum: null pointer");
+  CVVAE_CHECK_ARG(T >= 0 && H >= 1 && W >= 1 && 1ll * H * W < (1ll << 31),
+                  "cvvae_lpips_upsample_sum: needs T >= 0 and 1 <= H * W < 2^31, got T=%d H=%d W=%d", (int)T, (int)H, (int)W);
+  CVVAE_CHECK_ARG(reinterpret_cast<uintptr_t>(taps) % sizeof(double) == 0 && reinterpret_cast<uintptr_t>(out) % sizeof(float) == 0,
+                  "cvvae_lpips_upsample_sum: taps must be 8-byte and out 4-byte aligned");
+  LpTapMaps m;
+  long long off = 0;
+  for (int k = 0; k < kLpMaps; ++k) {
+    m.h[k] = tap_hw[2 * k];
+    m.w[k] = tap_hw[2 * k + 1];
+    CVVAE_CHECK_ARG(m.h[k] >= 1 && m.w[k] >= 1 && 1ll * m.h[k] * m.w[k] < (1ll << 31),
+                    "cvvae_lpips_upsample_sum: tap %d is %d x %d; needs 1 <= h * w < 2^31", k, (int)m.h[k], (int)m.w[k]);
+    m.off[k] = off;
+    off += 1ll * T * m.h[k] * m.w[k];
+  }
+  if (T == 0) return CVVAE_OK;
+  const long long n = 1ll * T * H * W;
+  const long long grid = (n + kLpUpThreads - 1) / kLpUpThreads;
+  CVVAE_CHECK_ARG(grid < (1ll << 31), "cvvae_lpips_upsample_sum: too many positions for one launch (T=%d at %d x %d)", (int)T,
+                  (int)H, (int)W);
+  lpips_upsample_sum_kernel<<<static_cast<unsigned>(grid), kLpUpThreads, 0, static_cast<cudaStream_t>(stream)>>>(taps, H, W, n,
+                                                                                                                 m, out);
+  CVVAE_LAUNCH_CHECK();
+  return CVVAE_OK;
 }
 
 extern "C" int cvvae_lpips_alex_input(const uint8_t* a_thwc, const uint8_t* b_thwc, int32_t T, int32_t H, int32_t W, float* out,

@@ -29,6 +29,10 @@
 // scaled by 16^j (a power of two, so no fp32 rounding changes).  In this mode a CTA
 // leaves, per colour channel, the sums of cs = (2 s_ab + C2) / (s_a^2 + s_b^2 + C2) and of the full SSIM, in units of
 // 2^-32; the channel of an output column is its element column mod 3.
+//
+// The SSIM map (cvvae_frame_ssim_map) is the byte instantiation with MAP set: every output element also stores its fp32
+// ssim, the value it rounds and sums, at map[t][r][c] with c its element column, so the map holds exactly the terms of the
+// frame's SSIM sum.  Consecutive threads own consecutive columns, so the stores of a row are coalesced.
 #include <math.h>
 
 #include <type_traits>
@@ -70,11 +74,13 @@ __device__ __forceinline__ uint4 load_vec16(uintptr_t q, uintptr_t lo, uintptr_t
 // E: uint8_t (frames) or uint16_t (MS-SSIM levels >= 1, sums of 4^j pixels); a row of a frame is WE = 3W elements.
 // MS false (cvvae_frame_metrics): acc[t] += {squared error, SSIM}.  MS true (one level of cvvae_frame_ms_ssim):
 // acc[t * 30 + 2 c] += {cs, SSIM} of channel c, with the elements shifted by `shift` = 128 * 4^j and C1, C2 = c1s, c2s.
-template <typename E, bool MS>
+// MAP (bytes, MS false; cvvae_frame_ssim_map): also map[(t (H - 10) + r) (WE - 30) + c] = ssim of output element (r, c).
+template <typename E, bool MS, bool MAP = false>
 __global__ void __launch_bounds__(kMetThreads)
     frame_metrics_kernel(const E* __restrict__ a, const E* __restrict__ b, int H, int WE, int tiles_x, int chunks_y,
                          long long total_bytes, MetWeights wt, unsigned long long* __restrict__ acc, int shift, float c1s,
-                         float c2s) {
+                         float c2s, float* __restrict__ map) {
+  static_assert(!MAP || (sizeof(E) == 1 && !MS), "the SSIM map is the byte, non-MS instantiation");
   using S = typename std::conditional<sizeof(E) == 1, int8_t, int16_t>::type;   // staged: element - shift
   constexpr int kVecs = met_vecs<E>(), kPitch = kVecs * 16;
   // rows of the open group, as element - shift (for bytes: stored as pixel ^ 0x80), each at its global 16-byte alignment:
@@ -190,6 +196,9 @@ __global__ void __launch_bounds__(kMetThreads)
             const float cs_d = __fadd_rn(__fadd_rn(va, vb), c2);
             const float ssim = __fdiv_rn(__fmul_rn(lum_n, cs_n), __fmul_rn(lum_d, cs_d));
             ssim_fix += __float2ll_rn(ssim * 4294967296.f);
+            if constexpr (MAP)
+              map[(static_cast<long long>(t) * (H - (kMetTaps - 1)) + r0 + g0 + j - (kMetTaps - 1)) * (WE - 2 * kMetHalo) + c0 +
+                  threadIdx.x] = ssim;
             if constexpr (MS) cs_fix += __float2ll_rn(__fdiv_rn(cs_n, cs_d) * 4294967296.f);
           }
         }
@@ -292,30 +301,44 @@ long long ms_level_bytes(int T, int H, int W, int j) {
   return (2ll * T * ms_extent(H, j) * ms_extent(W, j) * 3 + 255) / 256 * 256;
 }
 
+// The checks and launch shared by cvvae_frame_metrics (map NULL) and cvvae_frame_ssim_map (MAP, map required).
+template <bool MAP>
+int frame_metrics_launch(const char* who, const uint8_t* a_thwc, const uint8_t* b_thwc, int32_t T, int32_t H, int32_t W,
+                         int64_t* acc, float* map, void* stream_) {
+  CVVAE_CHECK_ARG(a_thwc && b_thwc && acc && (!MAP || map), "%s: null pointer", who);
+  CVVAE_CHECK_ARG(T >= 0 && H >= kMetTaps && W >= kMetTaps,
+                  "%s: needs T >= 0 and frames of at least 11 x 11 px, got T=%d H=%d W=%d", who, (int)T, (int)H, (int)W);
+  // sum over 3*H*W positions of ssim * 2^32 must stay inside int64
+  CVVAE_CHECK_ARG(3ll * H * W < (1ll << 31), "%s: %d x %d frames exceed the 64-bit accumulator's range (3*H*W < 2^31)", who,
+                  (int)H, (int)W);
+  CVVAE_CHECK_ARG(reinterpret_cast<uintptr_t>(map) % sizeof(float) == 0, "%s: `map` must be 4-byte aligned", who);
+  if (T == 0) return CVVAE_OK;
+  int tiles_x, chunks_y;
+  const long long grid = met_grid(T, H, W, &tiles_x, &chunks_y);
+  CVVAE_CHECK_ARG(grid < (1ll << 31), "%s: too many frames for one launch (T=%d at %d x %d)", who, (int)T, (int)H, (int)W);
+  const MetWeights wt = met_weights();
+
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  CVVAE_CUDA(cudaMemsetAsync(acc, 0, sizeof(int64_t) * 2 * T, stream));
+  frame_metrics_kernel<uint8_t, false, MAP><<<static_cast<unsigned>(grid), kMetThreads, 0, stream>>>(
+      a_thwc, b_thwc, H, 3 * W, tiles_x, chunks_y, 3ll * T * H * W, wt, reinterpret_cast<unsigned long long*>(acc), 128, 0.f, 0.f,
+      map);
+  CVVAE_LAUNCH_CHECK();
+  return CVVAE_OK;
+}
+
 }  // namespace cvvae
 
 using namespace cvvae;
 
 extern "C" int cvvae_frame_metrics(const uint8_t* a_thwc, const uint8_t* b_thwc, int32_t T, int32_t H, int32_t W, int64_t* acc,
-                                   void* stream_) {
-  CVVAE_CHECK_ARG(a_thwc && b_thwc && acc, "cvvae_frame_metrics: null pointer");
-  CVVAE_CHECK_ARG(T >= 0 && H >= kMetTaps && W >= kMetTaps,
-                  "cvvae_frame_metrics: needs T >= 0 and frames of at least 11 x 11 px, got T=%d H=%d W=%d", (int)T, (int)H, (int)W);
-  // sum over 3*H*W positions of ssim * 2^32 must stay inside int64
-  CVVAE_CHECK_ARG(3ll * H * W < (1ll << 31), "cvvae_frame_metrics: %d x %d frames exceed the 64-bit accumulator's range (3*H*W < 2^31)",
-                  (int)H, (int)W);
-  if (T == 0) return CVVAE_OK;
-  int tiles_x, chunks_y;
-  const long long grid = met_grid(T, H, W, &tiles_x, &chunks_y);
-  CVVAE_CHECK_ARG(grid < (1ll << 31), "cvvae_frame_metrics: too many frames for one launch (T=%d at %d x %d)", (int)T, (int)H, (int)W);
-  const MetWeights wt = met_weights();
+                                   void* stream) {
+  return frame_metrics_launch<false>("cvvae_frame_metrics", a_thwc, b_thwc, T, H, W, acc, nullptr, stream);
+}
 
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  CVVAE_CUDA(cudaMemsetAsync(acc, 0, sizeof(int64_t) * 2 * T, stream));
-  frame_metrics_kernel<uint8_t, false><<<static_cast<unsigned>(grid), kMetThreads, 0, stream>>>(
-      a_thwc, b_thwc, H, 3 * W, tiles_x, chunks_y, 3ll * T * H * W, wt, reinterpret_cast<unsigned long long*>(acc), 128, 0.f, 0.f);
-  CVVAE_LAUNCH_CHECK();
-  return CVVAE_OK;
+extern "C" int cvvae_frame_ssim_map(const uint8_t* a_thwc, const uint8_t* b_thwc, int32_t T, int32_t H, int32_t W, int64_t* acc,
+                                    float* map, void* stream) {
+  return frame_metrics_launch<true>("cvvae_frame_ssim_map", a_thwc, b_thwc, T, H, W, acc, map, stream);
 }
 
 extern "C" int64_t cvvae_ms_ssim_workspace_bytes(int32_t T, int32_t H, int32_t W) {
@@ -346,7 +369,7 @@ extern "C" int cvvae_frame_ms_ssim(const uint8_t* a_thwc, const uint8_t* b_thwc,
   CVVAE_CUDA(cudaMemsetAsync(acc, 0, sizeof(int64_t) * kMsLevels * 6 * T, stream));
 
   frame_metrics_kernel<uint8_t, true><<<static_cast<unsigned>(grid0), kMetThreads, 0, stream>>>(
-      a_thwc, b_thwc, H, 3 * W, tiles_x, chunks_y, 3ll * T * H * W, wt, out, 128, 6.5025f, 58.5225f);
+      a_thwc, b_thwc, H, 3 * W, tiles_x, chunks_y, 3ll * T * H * W, wt, out, 128, 6.5025f, 58.5225f, nullptr);
   CVVAE_LAUNCH_CHECK();
   // levels 1-4 of a, then of b, ...: a_1 | b_1 | a_2 | b_2 | ...
   uint8_t* ws = static_cast<uint8_t*>(workspace);
@@ -368,7 +391,7 @@ extern "C" int cvvae_frame_ms_ssim(const uint8_t* a_thwc, const uint8_t* b_thwc,
     const long long grid = met_grid(T, Hd, Wd, &tiles_x, &chunks_y);
     frame_metrics_kernel<uint16_t, true><<<static_cast<unsigned>(grid), kMetThreads, 0, stream>>>(
         la, lb, Hd, 3 * Wd, tiles_x, chunks_y, 6ll * T * Hd * Wd, wt, out + 6 * j, 128 << (2 * j), 6.5025f * scale,
-        58.5225f * scale);
+        58.5225f * scale, nullptr);
     CVVAE_LAUNCH_CHECK();
     prev_a = la;
     prev_b = lb;

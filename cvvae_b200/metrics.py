@@ -3,6 +3,7 @@
     frame_metrics(a, b)  ->  FrameMetrics(psnr, ssim, sse), host tensors with one entry per frame
     frame_ms_ssim(a, b)  ->  float64 host tensor with one MS-SSIM per frame
     LPIPS.from_state_dict(*state_dicts)(a, b)  ->  float64 host tensor with one LPIPS per frame
+    ssim_map(a, b), LPIPS.map(a, b)  ->  where they differ: per-position maps on the device (see the end)
 
 `a` and `b` are CUDA uint8 tensors [T, H, W, 3]: typically the frames the network saw (after the script's resize,
 cvvae_inference_video.py:28) and the frames it gave back (:47-50).  One kernel (`csrc/metrics.cu`) reads both once and
@@ -51,10 +52,24 @@ numbers).  Only the trunk differs: torchvision's ``alexnet().features[0:12]``, i
 padding 1) -> relu3 .. relu5, with C = 64, 192, 384, 256, 256 at the taps (``features[12]``, the last pool, is not
 part of LPIPS).  conv1 and conv2 run as 1 x 1 tensor-core convolutions over their taps packed into channels; the taps
 are h1 = (H - 7) // 4 + 1, p1 = (h1 - 3) // 2 + 1 for relu2, p2 = (p1 - 3) // 2 + 1 for relu3 .. relu5 (likewise W), so
-frames need at least 31 x 31 px.  The ``spatial=True`` variant (maps upsampled to the input size) is not provided.
+frames need at least 31 x 31 px.
+
+Maps say where two frames differ, not only how much:
+
+    ssim_map(a, b)  ->  CUDA float32 [T, H - 10, W - 10, 3], entry [t, y, x, c] the SSIM of channel c at pixel (y+5, x+5)
+    LPIPS.map(a, b)  ->  CUDA float32 [T, H, W], lpips' ``spatial=True``
+
+The SSIM map is written by the map instantiation of the PSNR / SSIM kernel: its entries are the fp32 values whose sum (in
+units of 2^-32) is the frame's SSIM, and the same launch leaves the same sums bit for bit.  The LPIPS map is each tap's
+head output sum_c w_k[c] (f^_a - f^_b)^2 per position (fp64), upsampled to H x W as ``nn.Upsample(size=(H, W),
+mode="bilinear", align_corners=False)`` upsamples an fp32 tensor, summed over the five taps in fp64 and rounded to fp32
+once.  Its mean is not exactly the scalar LPIPS (bilinear upsampling with clamped edges does not preserve the mean; the
+same holds for lpips).  Both are bit-reproducible and independent of how frames are grouped.
 """
 from __future__ import annotations
 
+import ctypes
+import functools
 from types import SimpleNamespace
 from typing import NamedTuple, Optional
 
@@ -82,13 +97,20 @@ class FrameMetrics(NamedTuple):
 
 
 @L._on_tensor_device
-def _launch(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
-    """The kernel on the current stream of the frames' device: int64 [T, 2] (sse, sum of ssim * 2^32), on the device."""
+def _launch(a: torch.Tensor, b: torch.Tensor, maps: bool = False):
+    """The kernel on the current stream of the frames' device: int64 [T, 2] (sse, sum of ssim * 2^32), on the device.
+    `maps`: the map instantiation of the same kernel, one launch, which also leaves the SSIM map: (sums, map fp32
+    [T, H - 10, W - 10, 3])."""
     T, H, W, _ = a.shape
     acc = torch.empty((T, 2), dtype=torch.int64, device=a.device)
-    L.check(L.load().cvvae_frame_metrics(a.data_ptr(), b.data_ptr(), T, H, W, acc.data_ptr(), L._stream(a)),
-            "cvvae_frame_metrics")
-    return acc
+    if not maps:
+        L.check(L.load().cvvae_frame_metrics(a.data_ptr(), b.data_ptr(), T, H, W, acc.data_ptr(), L._stream(a)),
+                "cvvae_frame_metrics")
+        return acc
+    out = torch.empty((T, H - _WINDOW + 1, W - _WINDOW + 1, 3), dtype=torch.float32, device=a.device)
+    L.check(L.load().cvvae_frame_ssim_map(a.data_ptr(), b.data_ptr(), T, H, W, acc.data_ptr(), out.data_ptr(), L._stream(a)),
+            "cvvae_frame_ssim_map")
+    return acc, out
 
 
 def _scores(acc: torch.Tensor, H: int, W: int) -> FrameMetrics:
@@ -110,9 +132,16 @@ def _check_frames(a: torch.Tensor, b: torch.Tensor, who: str) -> None:
 
 # A scorer is a metric as evaluate_frames runs it on every piece, and _sums for the per-frame functions (LPIPS is one):
 #   _check(H, W, who)     refuses a frame size before any device work (ValueError naming `who`)
-#   _launch(a, b)         the kernels on the frames' device and current stream: the int64 sums, on the device
+#   _launch(a, b)         the kernels on the frames' device and current stream: the int64 sums, on the device; or
+#                         (sums, *maps) for a scorer that also leaves maps, device tensors a piece carries as they are
 #   _finish(sums, H, W)   those sums on the host -> the float64 [T] tensors a piece of evaluate_frames carries
 #   _empty                the host sums of no frames
+# _with_maps(scorer) is the scorer whose _launch(a, b, maps=True) leaves its maps too.
+
+
+def _with_maps(scorer):
+    return SimpleNamespace(_check=scorer._check, _launch=functools.partial(scorer._launch, maps=True),
+                           _finish=scorer._finish, _empty=scorer._empty)
 
 
 def _sums(metric, a: torch.Tensor, b: torch.Tensor, who: str) -> torch.Tensor:
@@ -122,13 +151,30 @@ def _sums(metric, a: torch.Tensor, b: torch.Tensor, who: str) -> torch.Tensor:
     return metric._launch(a.contiguous(), b.contiguous()).cpu() if T else metric._empty
 
 
+def _check_ssim_size(H: int, W: int, who: str) -> None:
+    if H < _WINDOW or W < _WINDOW:
+        raise ValueError(f"{who}: SSIM needs frames of at least {_WINDOW} x {_WINDOW} px; got {H} x {W}")
+
+
 def frame_metrics(a: torch.Tensor, b: torch.Tensor) -> FrameMetrics:
     """PSNR, SSIM and squared error of every frame of `b` against the same frame of `a` (both CUDA uint8 [T, H, W, 3])."""
     _check_frames(a, b, "frame_metrics")
     _, H, W, _ = a.shape
-    if H < _WINDOW or W < _WINDOW:
-        raise ValueError(f"frame_metrics: SSIM needs frames of at least {_WINDOW} x {_WINDOW} px; got {H} x {W}")
+    _check_ssim_size(H, W, "frame_metrics")
     return _scores(_sums(_PSNR_SSIM, a, b, "frame_metrics"), H, W)
+
+
+def ssim_map(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
+    """The SSIM map of every frame of `b` against the same frame of `a` (both CUDA uint8 [T, H, W, 3], H, W >= 11): CUDA
+    float32 [T, H - 10, W - 10, 3] on the frames' device, entry [t, y, x, c] the SSIM of channel c under the 11 x 11
+    window centred on pixel (y + 5, x + 5).  Each entry is the fp32 value ``frame_metrics`` rounds to 2^-32 and sums, so
+    the frame's SSIM is the mean of the map up to that rounding.  One kernel launch."""
+    _check_frames(a, b, "ssim_map")
+    T, H, W, _ = a.shape
+    _check_ssim_size(H, W, "ssim_map")
+    if not T:
+        return torch.empty((0, H - _WINDOW + 1, W - _WINDOW + 1, 3), dtype=torch.float32, device=a.device)
+    return _launch(a.contiguous(), b.contiguous(), maps=True)[1]
 
 
 # evaluate_frames refuses no size for PSNR / SSIM on arrival: frame_metrics checks the 11 px itself, and in the stream
@@ -415,24 +461,30 @@ class LPIPS:
             dev = torch.device("cuda", torch.cuda.current_device() if dev is None or dev.index is None else dev.index)
         return cls(convs, heads, dev, net)
 
-    def _group(self, H: int, W: int) -> int:
+    def _group(self, H: int, W: int, maps: bool = False) -> int:
         """Frames per group: the budget over a frame pair's largest live activations (VGG16: conv1_2's input and output;
-        AlexNet: conv1's or conv2's)."""
-        return max(1, self._group_bytes // _NETS[self.net].pair_bytes(H, W))
+        AlexNet: conv1's or conv2's), plus with `maps` the frame's fp64 tap maps and its fp32 map."""
+        net = _NETS[self.net]
+        per_frame = net.pair_bytes(H, W)
+        if maps:
+            per_frame += 8 * sum(h * w for h, w in net.tap_sizes(H, W)) + 4 * H * W
+        return max(1, self._group_bytes // per_frame)
 
     def _check(self, H: int, W: int, who: str) -> None:
         _check_lpips_size(H, W, who, self.net)
 
     @L._on_tensor_device
-    def _launch(self, a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
+    def _launch(self, a: torch.Tensor, b: torch.Tensor, maps: bool = False):
         """The kernels on the current stream of the frames' device: int64 [5, T] (per tap and frame, the sum over
-        positions of the weighted squared difference times 2^32), on the device."""
+        positions of the weighted squared difference times 2^32), on the device.  `maps`: the same sums and the LPIPS
+        map, (sums, map fp32 [T, H, W]), from the same pass of the network."""
         T, H, W, _ = a.shape
         acc = torch.empty((len(_NETS[self.net].channels), T), dtype=torch.int64, device=a.device)
-        g = self._group(H, W)
+        out = torch.empty((T, H, W), dtype=torch.float32, device=a.device) if maps else None
+        g = self._group(H, W, maps)
         for t0 in range(0, T, g):
-            self._run_group(a[t0:t0 + g], b[t0:t0 + g], acc[:, t0:t0 + g])
-        return acc
+            self._run_group(a[t0:t0 + g], b[t0:t0 + g], acc[:, t0:t0 + g], None if out is None else out[t0:t0 + g])
+        return acc if out is None else (acc, out)
 
     def _finish(self, sums: torch.Tensor, H: int, W: int) -> tuple:
         return (_lpips_scores(sums, H, W, self.net),)
@@ -441,11 +493,17 @@ class LPIPS:
     def _empty(self) -> torch.Tensor:
         return torch.empty((len(_NETS[self.net].channels), 0), dtype=torch.int64)
 
-    def _run_group(self, a: torch.Tensor, b: torch.Tensor, acc: torch.Tensor) -> None:
+    def _run_group(self, a: torch.Tensor, b: torch.Tensor, acc: torch.Tensor, out: Optional[torch.Tensor] = None) -> None:
         """The network's plan on one group of frame pairs, both videos as one batch of 2G images.  Only the activation
-        the next step reads stays alive: each step's output replaces it, a tap without a side output leaves it."""
+        the next step reads stays alive: each step's output replaces it, a tap without a side output leaves it.
+        `out` (fp32 [G, H, W]): the taps also leave their maps, fp64 and back to back, and one launch after the plan
+        upsamples and sums them into it."""
         G, H, W, _ = a.shape
         net, lib, stream = _NETS[self.net], self._ops.lib, L._stream(a)
+        sizes = net.tap_sizes(H, W)
+        if out is not None:
+            taps = torch.empty(G * sum(h * w for h, w in sizes), dtype=torch.float64, device=a.device)
+            offsets = [G * sum(h * w for h, w in sizes[:k]) for k in range(len(sizes))]
         x = None
         for (op, *arg), shape in zip(net.plan, net.shapes(H, W)):
             y = (None if op == "tap" and arg[1] is None else
@@ -458,14 +516,41 @@ class LPIPS:
                 self._ops.conv(x, wp, bias, out=y, relu=True, tf32_out=arg[1], **kw)
             elif op == "tap":
                 k, side = arg
-                fn = "cvvae_lpips_tap_copy" if side == "copy" else "cvvae_lpips_tap"
-                L.check(getattr(lib, fn)(x.data_ptr(), G, *x.shape[2:], self._heads[k].data_ptr(), acc[k].data_ptr(),
-                                         None if y is None else y.data_ptr(), stream), fn)
+                y_ptr = None if y is None else y.data_ptr()
+                args = (x.data_ptr(), G, *x.shape[2:], self._heads[k].data_ptr(), acc[k].data_ptr())
+                if out is not None:
+                    fn = "cvvae_lpips_tap_map"
+                    sides = (None, y_ptr) if side == "copy" else (y_ptr, None)
+                    L.check(lib.cvvae_lpips_tap_map(*args, *sides, taps[offsets[k]:].data_ptr(), stream), fn)
+                else:
+                    fn = "cvvae_lpips_tap_copy" if side == "copy" else "cvvae_lpips_tap"
+                    L.check(getattr(lib, fn)(*args, y_ptr, stream), fn)
             else:   # max_pool3s2, pack5x5: image by image
                 fn = "cvvae_lpips_" + op
                 L.check(getattr(lib, fn)(x.data_ptr(), 2 * G, *x.shape[2:], y.data_ptr(), stream), fn)
             if y is not None:
                 x = y
+        if out is not None:
+            hw = (ctypes.c_int32 * (2 * len(sizes)))(*(n for size in sizes for n in size))
+            L.check(lib.cvvae_lpips_upsample_sum(taps.data_ptr(), G, H, W, hw, out.data_ptr(), stream),
+                    "cvvae_lpips_upsample_sum")
+
+    def map(self, a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
+        """The LPIPS map of every frame of `b` against the same frame of `a`, lpips' ``spatial=True``: CUDA float32
+        [T, H, W] on ``metric.device``, with the inputs and limits of ``metric(a, b)``.  Each tap's head output
+        sum_c w_k[c] (f^_a - f^_b)^2 is kept per position (fp64), upsampled to H x W as ``nn.Upsample(size=(H, W),
+        mode="bilinear", align_corners=False)`` does for fp32 tensors, and the five are summed in fp64 and rounded to
+        fp32 once.  The map's mean is close to, but not exactly, the scalar LPIPS: bilinear upsampling with the edges
+        clamped does not preserve the mean (lpips' spatial maps behave the same way).  One pass of the network gives both:
+        ``metric.launches + 1`` launches per group of frames, and the map is the same, bit for bit, whatever the grouping."""
+        _check_frames(a, b, "LPIPS.map")
+        if a.device != self.device:
+            raise ValueError(f"LPIPS.map: the frames are on {a.device}, the weights on {self.device}")
+        T, H, W, _ = a.shape
+        self._check(H, W, "LPIPS.map")
+        if not T:
+            return torch.empty((0, H, W), dtype=torch.float32, device=a.device)
+        return self._launch(a.contiguous(), b.contiguous(), maps=True)[1]
 
     def __call__(self, a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
         _check_frames(a, b, "LPIPS")

@@ -235,7 +235,8 @@ def reconstruct_frames(model, frames: Iterable, size=None, sample_posterior: boo
 
 
 def evaluate_frames(model, frames: Iterable, size=None, sample_posterior: bool = False,
-                    generator: Optional[torch.Generator] = None, *, ms_ssim: bool = False, lpips=None) -> Iterator[tuple]:
+                    generator: Optional[torch.Generator] = None, *, ms_ssim: bool = False, lpips=None,
+                    maps: bool = False) -> Iterator[tuple]:
     """``reconstruct_frames`` with a score for every frame: yields ``(frames_u8, psnr, ssim)`` per piece,
     ``(frames_u8, psnr, ssim, ms_ssim)`` with ``ms_ssim=True``, and the per-frame LPIPS as one more last element when
     `lpips` is given.
@@ -262,15 +263,27 @@ def evaluate_frames(model, frames: Iterable, size=None, sample_posterior: bool =
     frames; its sums ride in the same download.  The activations of one group are freed before the next, so device
     memory stays flat in the clip's length.  LPIPS needs frames of at least ``lpips.min_size`` px on each side as the
     network sees them (16 for VGG16, 31 for AlexNet); smaller ones raise ``ValueError`` when the first of them arrives.
+
+    ``maps=True`` says where each frame lost, not only how much: after every element above, each piece also carries the
+    SSIM map (``metrics.ssim_map``, host float32 ``[t', h - 10, w - 10, 3]``) and, when `lpips` is given, the LPIPS map
+    (``LPIPS.map``, host float32 ``[t', h, w]``), scored against the same aligned input frames.  The PSNR / SSIM launch
+    becomes the kernel's map instantiation (still one launch, the same sums bit for bit) and LPIPS runs its network once
+    for both score and map; the maps ride in the same download, so device memory stays flat in the clip's length.  The
+    download grows accordingly: at 576 x 1024 the maps are 6.9 MB (SSIM) and 2.4 MB (LPIPS) per frame, against 1.8 MB for
+    the uint8 frame.  Anything but a bool for `maps` raises ``ValueError``.
     """
     from . import metrics
+    if not isinstance(maps, bool):
+        raise ValueError(f"evaluate_frames: `maps` must be a bool; got {maps!r}")
     if lpips is not None:
         if not isinstance(lpips, metrics.LPIPS):
             raise ValueError(f"evaluate_frames: `lpips` must be a metrics.LPIPS or None; got {type(lpips).__name__}")
         if lpips.device != model.device:
             raise ValueError(f"evaluate_frames: the LPIPS weights are on {lpips.device}, the model on {model.device}")
     enc, dec = _open(model, "evaluate_frames")
-    scorers = [metrics._PSNR_SSIM] + ([metrics._MS_SSIM] if ms_ssim else []) + ([lpips] if lpips is not None else [])
+    mapped = metrics._with_maps if maps else (lambda scorer: scorer)
+    scorers = ([mapped(metrics._PSNR_SSIM)] + ([metrics._MS_SSIM] if ms_ssim else []) +
+               ([mapped(lpips)] if lpips is not None else []))
     return _reconstruct(model, enc, dec, iter(frames), size, sample_posterior, generator, scorers)
 
 
@@ -285,7 +298,7 @@ def _open(model, who: str):
 def _reconstruct(model, enc: StreamEncoder, dec: StreamDecoder, frames: Iterator, size, sample_posterior: bool,
                  generator, scorers: list) -> Iterator:
     """The stream behind reconstruct_frames (no `scorers`: yields frames) and evaluate_frames (yields the frames, then
-    what each of `scorers`, metrics' scorers, finishes for them)."""
+    what each of `scorers`, metrics' scorers, finishes for them, then the maps they leave, in the same order)."""
     from .video_io import frames_to_input, frames_to_input_and_u8, output_to_frames
 
     # No device context is held across the yields (it would leak into the caller's code): every allocation, stream and
@@ -318,13 +331,15 @@ def _reconstruct(model, enc: StreamEncoder, dec: StreamDecoder, frames: Iterator
             raise ValueError(f"evaluate_frames: the networks return {u8.shape[1]} x {u8.shape[2]} frames for an input of "
                              f"{ref.shape[1]} x {ref.shape[2]}, and frames of different sizes cannot be scored; pass "
                              "`size=` with a size the networks reproduce (a multiple of their spatial stride)")
-        io.download(u8, *[m._launch(ref, u8) for m in scorers])
+        left = [out if isinstance(out, tuple) else (out,) for out in (m._launch(ref, u8) for m in scorers)]
+        io.download(u8, *[out[0] for out in left], *[v for out in left for v in out[1:]])   # the sums, then the maps
 
-    def piece(host: torch.Tensor, *sums: torch.Tensor):
+    def piece(host: torch.Tensor, *outs: torch.Tensor):
         if not scorers:
             return host
         H, W = host.shape[1], host.shape[2]
-        return (host,) + tuple(v for m, s in zip(scorers, sums) for v in m._finish(s, H, W))
+        sums, maps = outs[:len(scorers)], outs[len(scorers):]
+        return (host,) + tuple(v for m, s in zip(scorers, sums) for v in m._finish(s, H, W)) + maps
 
     def decode_chunks(latent_chunks) -> None:
         for post in latent_chunks:

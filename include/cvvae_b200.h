@@ -239,6 +239,13 @@ int cvvae_video_train_input(const uint8_t* thwc, void* out_cthw, int32_t T, int3
  * T >= 0 (T == 0 launches nothing), H, W >= 11 and 3*H*W < 2^31, else CVVAE_E_ARG.  One kernel launch. */
 int cvvae_frame_metrics(const uint8_t* a_thwc, const uint8_t* b_thwc, int32_t T, int32_t H, int32_t W, int64_t* acc,
                         void* stream);
+/* cvvae_frame_metrics that also writes the SSIM map: map fp32 [T][H-10][3(W-10)], 4-byte aligned, overwritten with
+ * map[t][y][3x + c] = the ssim above of channel c at pixel (y+5, x+5), the exact fp32 value whose llrint(ssim * 2^32) the
+ * SSIM sum adds, so that sum over the map of llrint(v * 2^32) == acc[t][1].  acc is computed exactly as by
+ * cvvae_frame_metrics, bit for bit.  The refusals of cvvae_frame_metrics, plus a NULL or misaligned map (CVVAE_E_ARG,
+ * before any launch).  One kernel launch. */
+int cvvae_frame_ssim_map(const uint8_t* a_thwc, const uint8_t* b_thwc, int32_t T, int32_t H, int32_t W, int64_t* acc,
+                         float* map, void* stream);
 /* Multi-scale SSIM (Wang, Simoncelli and Bovik 2003) of the same two videos, as per-level sums; the caller combines them.
  * Level 0 is the frames; level j+1 is the 2x2 average pool of level j, an odd extent zero-padded in front (output i of an
  * axis of odd length covers inputs 2i-1 and 2i, input -1 being 0; the divisor stays 4).  At each level j = 0..4, per
@@ -316,6 +323,24 @@ int cvvae_lpips_max_pool3s2(const float* f, int32_t N, int32_t H, int32_t W, int
 int cvvae_lpips_pack5x5(const float* x, int32_t N, int32_t H, int32_t W, int32_t C, float* out, void* stream);
 int cvvae_lpips_tap_copy(const float* f, int32_t T, int32_t H, int32_t W, int32_t C, const float* lin_w, int64_t* acc,
                          float* copy, void* stream);
+/* LPIPS maps (lpips spatial=True) for either network:
+ *   cvvae_lpips_tap_map: cvvae_lpips_tap with `pooled` (VGG16's taps 1-4) or cvvae_lpips_tap_copy with `copy` (AlexNet's
+ *     relu3, relu4), at most one of them set, else CVVAE_E_ARG; the same checks, the same acc bit for bit, the same side
+ *     output.  It also writes map fp64 [T,H,W], 8-byte aligned (NULL or misaligned: CVVAE_E_ARG):
+ *       map[t][h][w] = sum_c w[c] (fa_c / n_a - fb_c / n_b)^2 at that position, its own fp64 sum (not the fixed-point one),
+ *     so that the mean of map[t] is d_k(t) up to the rounding of acc.  One launch (plus a memset of acc).
+ *   cvvae_lpips_upsample_sum: taps fp64, the five tap maps [T,h_k,w_k] back to back (tap k from element
+ *     sum_{j<k} T h_j w_j), tap_hw host int32 [10] = h_0, w_0, .., h_4, w_4 -> out fp32 [T,H,W] = sum over k of tap map k
+ *     upsampled to H x W as nn.Upsample(size=(H, W), mode='bilinear', align_corners=False) does for fp32 tensors: per axis
+ *     scale = (float)in / out, src = max(scale (dst + 0.5) - 0.5, 0) in fp32, i0 = (int)src, i1 = i0 + (i0 < in - 1),
+ *     lambda = src - i0; the interpolation and the sum over k are fp64, rounded to fp32 once.  taps 8-byte and out 4-byte
+ *     aligned; T >= 0 (T == 0 launches nothing), 1 <= H*W < 2^31, 1 <= h_k*w_k < 2^31, else CVVAE_E_ARG.  One launch.
+ *   A group of frames then costs one launch more than its scores alone.  The map's mean over H x W is not exactly
+ *   sum_k d_k: bilinear upsampling with the edges clamped does not preserve the mean (lpips behaves the same way). */
+int cvvae_lpips_tap_map(const float* f, int32_t T, int32_t H, int32_t W, int32_t C, const float* lin_w, int64_t* acc,
+                        float* pooled, float* copy, double* map, void* stream);
+int cvvae_lpips_upsample_sum(const double* taps, int32_t T, int32_t H, int32_t W, const int32_t* tap_hw, float* out,
+                             void* stream);
 
 /* Diagnostics */
 /* Per-CTA phase timestamps of the next conv_tc launches: device buffer of n_ctas x 8 uint64 (globaltimer ns:

@@ -15,7 +15,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIBPATH = os.path.join(LIBDIR, "libcvvae_b200.so")
 SOURCES = ["api.cu", "conv_tc.cu", "conv_stk.cu", "conv_direct.cu", "groupnorm.cu", "attention.cu", "misc.cu", "video_io.cu",
-           "metrics.cu", "lpips.cu"]
+           "metrics.cu", "lpips.cu", "i3d.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC",

@@ -87,7 +87,12 @@ _SIGNATURES = {
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "cvvae_lpips_upsample_sum": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.c_void_p,
                                            C.c_void_p]),
-    "cvvae_conv_tc_set_trace": (C.c_int, [C.c_void_p, C.c_int32]),
+    "cvvae_i3d_stem_input": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "cvvae_i3d_max_pool3d": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                       C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_void_p, C.c_void_p]),
+    "cvvae_i3d_head": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                 C.c_int32, C.c_void_p, C.c_void_p]),
+    "cvvae_conv_tc_set_trace":(C.c_int, [C.c_void_p, C.c_int32]),
     "cvvae_conv_tc_plan": (C.c_int, [C.POINTER(ConvDesc), C.POINTER(C.c_int32), C.c_int32]),
     "cvvae_last_error": (C.c_char_p, []),
     "cvvae_abi_version": (C.c_int, []),

@@ -17,7 +17,8 @@ saw.
 ``encode_clips`` turns a dataset of clips into latents: each clip goes through the reference's training pre-processing
 (``video_io.frames_to_training_input``) straight into its slot of a batch, and batches of clips with equal length run
 through one ``model.encode`` call each.  ``decode_clips`` is the way back: batches of clip latents of equal shape run
-through one ``model.tiled_decode`` call and one pixel conversion each, and come back as uint8 videos.
+through one ``model.tiled_decode`` call and one pixel conversion each, and come back as uint8 videos.  ``embed_clips``
+scores such sets: each clip's I3D embedding for FVD (``fvd.py``), batched the same way.
 """
 from __future__ import annotations
 
@@ -463,6 +464,69 @@ def _encode_clips(model, clips: Iterator, size: tuple, resize: str, batch_size: 
         io.download(moments)
         del moments
         # one-batch lag: a batch's moments go to the caller only once the next batch is enqueued behind it
+        while len(io) > 1:
+            yield from io.take()[0].unbind(0)
+    while io:
+        yield from io.take()[0].unbind(0)
+
+
+def embed_clips(i3d, clips: Iterable, batch_size: int = 16) -> Iterator[torch.Tensor]:
+    """FVD's I3D embedding of every clip of a dataset, batched on the GPU (``fvd.I3D``, ``fvd.frechet_distance``).
+
+    `clips` is an iterable of uint8 clips ``[T, H, W, 3]`` with T >= 9: numpy arrays, CPU tensors or tensors on the
+    network's device; T and the source size may differ from clip to clip.  Yields, for each clip in input order, a host
+    float64 tensor ``[K]`` (K = 400 for Kinetics-400) equal bit for bit to ``i3d(clip[None])[0]``.
+
+    Consecutive clips of equal ``(T, H, W)`` are stacked into one batch of at most `batch_size` (``clip_batches``); host
+    clips are uploaded through a side stream, each clip is prepared into its slot of the batch by one
+    ``frames_to_training_input(..., size=224, resize="short", dtype=torch.float32, out=...)`` launch, and the batch runs
+    through the network in groups of ``i3d.group(T)`` clips.  A batch's embeddings are yielded once the next batch has
+    been enqueued.  Device memory holds one batch's prepared clips and one group's activations plus the clips in flight,
+    however many clips there are.
+
+    Raises ValueError at the call for anything but an ``I3D`` or a `batch_size` that is not an int >= 1, and when an item
+    arrives that is not a uint8 ``[T, H, W, 3]`` clip with T >= 9 on the host or the network's device."""
+    from .fvd import I3D
+    if not isinstance(i3d, I3D):
+        raise ValueError(f"embed_clips: `i3d` must be an fvd.I3D; got {type(i3d).__name__}")
+    if isinstance(batch_size, bool) or not isinstance(batch_size, int) or batch_size < 1:
+        raise ValueError(f"embed_clips: batch_size must be an int >= 1; got {batch_size!r}")
+    return _embed_clips(i3d, iter(clips), batch_size)
+
+
+def _embed_clip(item, device: torch.device) -> torch.Tensor:
+    """One clip (numpy array or tensor) as a host or `device` uint8 tensor [T, H, W, 3] with T >= 9; ValueError otherwise."""
+    from .fvd import I3D_MIN_FRAMES
+    item = torch.as_tensor(item)
+    if (item.dtype != torch.uint8 or item.dim() != 4 or item.shape[0] < I3D_MIN_FRAMES or item.shape[-1] != 3
+            or min(item.shape[1:3]) < 1):
+        raise ValueError(f"embed_clips expects uint8 clips [T, H, W, 3] with T >= {I3D_MIN_FRAMES}; got {item.dtype} "
+                         f"{tuple(item.shape)}")
+    if item.device.type != "cpu" and item.device != device:
+        raise ValueError(f"embed_clips: a clip on {item.device} for a network on {device}; pass host tensors or tensors "
+                         "on the network's device")
+    return item
+
+
+def _embed_clips(i3d, clips: Iterator, batch_size: int) -> Iterator[torch.Tensor]:
+    from .fvd import I3D_SIZE
+    from .video_io import frames_to_training_input
+
+    dev = i3d.device
+    checked = (_embed_clip(item, dev) for item in clips)
+    # As in _encode_clips, no device context is held across the yields, and the `del`s keep device memory one batch deep.
+    io = _HostTransfers(dev)
+    for batch in clip_batches(checked, batch_size, length=lambda clip: tuple(clip.shape[:3])):
+        x = torch.empty((len(batch), 3, batch[0].shape[0], I3D_SIZE, I3D_SIZE), dtype=torch.float32, device=dev)
+        for i, clip in enumerate(batch):
+            src = io.upload(clip) if clip.device.type == "cpu" else clip
+            frames_to_training_input(src, I3D_SIZE, "short", torch.float32, out=x[i:i + 1])
+            del src
+        emb = i3d._embed(x)
+        del x
+        io.download(emb)
+        del emb
+        # one-batch lag: a batch's embeddings go to the caller only once the next batch is enqueued behind it
         while len(io) > 1:
             yield from io.take()[0].unbind(0)
     while io:

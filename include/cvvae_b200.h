@@ -342,6 +342,33 @@ int cvvae_lpips_tap_map(const float* f, int32_t T, int32_t H, int32_t W, int32_t
 int cvvae_lpips_upsample_sum(const double* taps, int32_t T, int32_t H, int32_t W, const int32_t* tap_hw, float* out,
                              void* stream);
 
+/* FVD's network: the Kinetics-400 I3D (InceptionI3d of the common PyTorch port) in fp32 with TF32 products, on N clips.
+ * TF "SAME" padding per axis of extent n, kernel k, stride s: pad = max(k - s, 0) if n % s == 0 else max(k - n % s, 0),
+ * front = pad / 2; the output extent is ceil(n / s).  The caller runs:
+ *   cvvae_i3d_stem_input: x fp32 [N,3,T,H,W] contiguous (frames_to_training_input's output, 4-byte aligned) -> out fp32
+ *     [N,TP,OH,OW,448] channels-last, 16-byte aligned, TP = ceil(T/2) + 2, OH = ceil(H/2), OW = ceil(W/2).  Channel
+ *     ((j*7 + kh)*7 + kw)*3 + c of (u, oh, ow) is x(c, 2u - ft + j, 2oh - fh + kh, 2ow - fw + kw), j < 3, with ft, fh, fw the
+ *     SAME front paddings of Conv3d_1a_7x7 (k = 7, s = 2), stored rounded to the nearest TF32 value; 0 outside the clip and
+ *     in channels 441..447.  Conv3d_1a_7x7 then runs as a 3 x 1 x 1 stride-1 convolution (no offset) over these 448
+ *     channels whose tap k holds the temporal taps 2k + j (tap 0: j = 0, 1, 2; taps 1 and 2: j = 1, 2; every other
+ *     weight zero).  N >= 0 (N == 0 launches nothing), T, H, W >= 1, TP*OH*OW*112 < 2^31.  One launch.
+ *   The 57 BN-folded convolutions (conv3d, BatchNorm3d(eps=1e-3) in eval mode, ReLU) through cvvae_conv3d with
+ *     CVVAE_CONV_RELU and SAME offsets, plus CVVAE_CONV_TF32_OUT on all but Mixed_5c's branches (the head reads those).
+ *   cvvae_i3d_max_pool3d: f fp32 [N,T,H,W,C] -> out fp32 [N,ceil(T/st),ceil(H/sh),ceil(W/sw),C], both channels-last,
+ *     contiguous and 16-byte aligned, kernel / stride host int32 [3] (t, h, w), each 1..7: the maximum over the window with
+ *     SAME zero padding (a tap outside the input counts as 0), an exact copy of the winning value.  N >= 0, T, H, W >= 1,
+ *     C % 4 == 0, T*H*W*C < 2^31.  One launch.
+ *   cvvae_i3d_head: f fp32 [N,T,7,7,C] (Mixed_5c, T >= 2), w fp32 [K][C] and bias fp32 [K] (the logits convolution) ->
+ *     out fp64 [N,K] = bias + w . m, m[c] the mean over the T - 1 positions of AvgPool3d([2,7,7], stride 1) of channel c;
+ *     all arithmetic fp64, bit-reproducible and independent of the other clips.  1 <= C <= 4096, K >= 1; out 8-byte
+ *     aligned.  One launch.
+ * Every refusal is CVVAE_E_ARG before any launch. */
+int cvvae_i3d_stem_input(const float* x, int32_t N, int32_t T, int32_t H, int32_t W, float* out, void* stream);
+int cvvae_i3d_max_pool3d(const float* f, int32_t N, int32_t T, int32_t H, int32_t W, int32_t C, const int32_t* kernel,
+                         const int32_t* stride, float* out, void* stream);
+int cvvae_i3d_head(const float* f, int32_t N, int32_t T, int32_t H, int32_t W, int32_t C, const float* w, const float* bias,
+                   int32_t K, double* out, void* stream);
+
 /* Diagnostics */
 /* Per-CTA phase timestamps of the next conv_tc launches: device buffer of n_ctas x 8 uint64 (globaltimer ns:
  * entry, setup done, first A landed, first B landed, all MMAs issued, accumulators ready, epilogue done,
